@@ -183,6 +183,12 @@ pp_status pp_gemm_stats_geometry(const pp_gemm_desc* d, pp_stats_geom* out);
 int64_t pp_gemm_splitk_bytes(const pp_gemm_desc* d, int32_t* tiles_out);
 /* host-only query: number of per-row LayerNorm records this GEMM emits through row_stats (0: it cannot emit them) */
 int32_t pp_gemm_row_stats_records(const pp_gemm_desc* d);
+/* host-only query: the kernel variant pp_gemm_conv would launch for this descriptor: tile width (64/128/160/256),
+   epilogue mode (0 plain bf16, 1 generic, 2 GEGLU, 3 LayerNorm-statistics producer, 4 LayerNorm-folded consumer,
+   5 transposed columns through the staging tile) and split-K factor (1 or 2; 2 runs the mode-0 split-K kernel).
+   It validates the shape and the tile width only: the answer is the launch's for a descriptor pp_gemm_conv accepts
+   (e.g. row_stats together with ln_stats reports mode 3, while pp_gemm_conv refuses that descriptor) */
+pp_status pp_gemm_variant(const pp_gemm_desc* d, int32_t* block_n, int32_t* mode, int32_t* ksplit);
 
 /* ------------------------------------------------------------------ attention */
 typedef struct pp_attn_desc {
@@ -201,6 +207,9 @@ typedef struct pp_attn_desc {
 } pp_attn_desc;
 
 pp_status pp_attention(const pp_attn_desc* d, pp_stream stream);
+/* host-only query: the kernel variant pp_attention would launch: PV width dv (d rounded up to one of
+   32/48/64/80/96/128/160/192) and whether P is fp16 (vt_fp16) or bf16 */
+pp_status pp_attention_variant(const pp_attn_desc* d, int32_t* dv, int32_t* p_fp16);
 
 /* ------------------------------------------------------------------ norms */
 typedef struct pp_gn_desc {

@@ -111,7 +111,9 @@ _SIGNATURES = {
     "pp_gemm_stats_geometry": (C.c_int, [C.POINTER(GemmDesc), C.POINTER(StatsGeom)]),
     "pp_gemm_row_stats_records": (i32, [C.POINTER(GemmDesc)]),
     "pp_gemm_splitk_bytes": (i64, [C.POINTER(GemmDesc), C.POINTER(i32)]),
+    "pp_gemm_variant": (C.c_int, [C.POINTER(GemmDesc), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
     "pp_attention": (C.c_int, [C.POINTER(AttnDesc), vp]),
+    "pp_attention_variant": (C.c_int, [C.POINTER(AttnDesc), C.POINTER(i32), C.POINTER(i32)]),
     "pp_group_norm": (C.c_int, [C.POINTER(GnDesc), vp]),
     "pp_group_norm_scratch_bytes": (i64, [i32, i32, i32, i32]),
     "pp_layer_norm": (C.c_int, [vp, vp, vp, vp, i32, i32, f32, vp]),

@@ -240,6 +240,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
 // instantiated PV widths: the head dim is rounded up to the next of these (SD-1.5: d = 40 / 80 / 160)
 static constexpr int ATT_DVS[8] = {32, 48, 64, 80, 96, 128, 160, 192};
 
+// index into ATT_DVS of the PV width a head dim d (8..192) runs at. Shared by attn_prepare and pp_attention_variant.
+static int att_dv_index(int d) {
+    int dvi = 0;
+    while (dvi < 7 && ATT_DVS[dvi] < d) ++dvi;
+    return dvi;
+}
+
 template <int DV, bool F16>
 static int attn_ensure_attr() {
     static bool done[PP_MAX_DEVICES] = {};  // the attribute is per device
@@ -300,8 +307,7 @@ int attn_prepare(const pp_attn_desc& d, AttnLaunch* out) {
     PP_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "attention: out not 16-byte aligned");
     p.batch = d.batch; p.heads = d.heads; p.d = d.d; p.nq = d.nq; p.nk = d.nk;
     p.k_steps = (d.d + 15) / 16;
-    int dvi = 0;
-    while (ATT_DVS[dvi] < d.d) ++dvi;
+    const int dvi = att_dv_index(d.d);
     p.dv = ATT_DVS[dvi];
     p.scale_log2 = d.scale * 1.4426950408889634f;
     p.vt_fp16 = d.vt_fp16;
@@ -345,6 +351,20 @@ int attn_launch(const AttnLaunch& l, cudaStream_t s) {
 }
 
 }  // namespace pp
+
+extern "C" pp_status pp_attention_variant(const pp_attn_desc* d, int32_t* dv, int32_t* p_fp16) {
+    if (!d || !dv || !p_fp16) {
+        pp::set_last_error("pp_attention_variant: null argument");
+        return pp::PP_ERR_INVALID;
+    }
+    if (d->d < 8 || d->d % 8 != 0 || d->d > 192) {
+        pp::set_last_error("attention: head dim %d unsupported (multiple of 8, <= 192)", d->d);
+        return pp::PP_ERR_INVALID;
+    }
+    *dv = pp::ATT_DVS[pp::att_dv_index(d->d)];
+    *p_fp16 = d->vt_fp16 ? 1 : 0;
+    return pp::PP_OK;
+}
 
 extern "C" pp_status pp_attention(const pp_attn_desc* d, pp_stream stream) {
     if (!d) {

@@ -1255,7 +1255,6 @@ static int ensure_attr() {
         case 128 * 8 + 2: return FN<128, 2>(__VA_ARGS__);                        \
         case 160 * 8 + 0: return FN<160, 0>(__VA_ARGS__);                        \
         case 160 * 8 + 1: return FN<160, 1>(__VA_ARGS__);                        \
-        case 160 * 8 + 2: return FN<160, 2>(__VA_ARGS__);                        \
         case 256 * 8 + 0: return FN<256, 0>(__VA_ARGS__);                        \
         case 256 * 8 + 1: return FN<256, 1>(__VA_ARGS__);                        \
         case 256 * 8 + 2: return FN<256, 2>(__VA_ARGS__);                        \
@@ -1397,6 +1396,10 @@ static int gemm_geometry(const pp_gemm_desc& d, GemmKParams& p, int* block_n_out
         }
     }
     PP_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256, "gemm: block_n %d unsupported", bn);
+    if (geglu) {
+        PP_REQUIRE(d.N % bn == 0, "gemm: GEGLU needs N %% block_n == 0 (N=%d, block_n=%d)", d.N, bn);
+        PP_REQUIRE(bn == 128 || bn == 256, "gemm: GEGLU block_n must be 128 or 256 (got %d)", bn);
+    }
     p.m_tiles = m_tiles;
     p.n_tiles = ceil_div(d.N, bn);
     *block_n_out = bn;
@@ -1454,6 +1457,28 @@ int gemm_row_stats_records(const pp_gemm_desc& d0) {
     if (gemm_geometry(d, p, &bn)) return 0;
     if (d.a_mode != PP_A_MATRIX || !gemm_fast_mode(d) || d.act != PP_ACT_NONE) return 0;
     return 2 * p.n_tiles;
+}
+
+// Epilogue flavour (the MODE template argument) of a launch: 2 GEGLU, 5 transposed columns through the staging tile,
+// 3 / 4 / 0 the fast bf16 epilogue (LayerNorm-statistics producer / LayerNorm-folded consumer / plain), 1 the generic
+// one. Shared by gemm_prepare and the host-only pp_gemm_variant.
+static int gemm_select_mode(const pp_gemm_desc& d) {
+    if (d.epilogue == PP_EPI_GEGLU) return 2;
+    if (gemm_trans_staged(d)) return 5;
+    if (gemm_fast_mode(d)) return d.row_stats ? 3 : d.ln_stats ? 4 : 0;
+    return 1;
+}
+
+int gemm_variant(const pp_gemm_desc& d, int* block_n, int* mode, int* ksplit) {
+    GemmKParams p;
+    memset(&p, 0, sizeof(p));
+    int bn = 0, ks = 1;
+    int rc = gemm_geometry(d, p, &bn, &ks);
+    if (rc) return rc;
+    *block_n = bn;
+    *mode = gemm_select_mode(d);
+    *ksplit = ks;
+    return PP_OK;
 }
 
 int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
@@ -1516,8 +1541,6 @@ int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
     }
     const bool geglu = d.epilogue == PP_EPI_GEGLU;
     if (geglu) {
-        PP_REQUIRE(d.N % bn == 0, "gemm: GEGLU needs N %% block_n == 0 (N=%d, block_n=%d)", d.N, bn);
-        PP_REQUIRE(bn == 128 || bn == 256, "gemm: GEGLU block_n must be 128 or 256 (got %d)", bn);
         PP_REQUIRE(!d.out_fp32 && !d.rowvec && !d.res1 && !d.res2, "gemm: GEGLU epilogue takes bias only");
         PP_REQUIRE(d.ldc % 8 == 0, "gemm: GEGLU ldc must be a multiple of 8");
     }
@@ -1582,10 +1605,8 @@ int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
         }
     }
     l.smem = smem_for_block_n(bn);
-    if (geglu) {
-        l.mode = 2;
-    } else if (gemm_trans_staged(d)) {
-        l.mode = 5;
+    l.mode = gemm_select_mode(d);
+    if (l.mode == 5) {
         const bool mixed = d.epilogue == PP_EPI_ROWS_THEN_TRANSPOSED;
         if (mixed)
             PP_REQUIRE(d.out_t && d.trans_from_col > 0 && d.trans_from_col < d.N && d.trans_from_col % bn == 0 &&
@@ -1604,11 +1625,10 @@ int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
             int rc = make_tmap_bf16_sw(&p.tmOutT[k], out_t, 3, dims, str, box, 0);
             if (rc) return rc;
         }
-    } else {
+    } else if (l.mode != 2) {
         PP_REQUIRE(d.epilogue != PP_EPI_ROWS_THEN_TRANSPOSED, "gemm: PP_EPI_ROWS_THEN_TRANSPOSED needs a plain bf16 GEMM "
                    "(bias only) whose t_rows is a multiple of 128 and divides M");
         PP_REQUIRE(!(d.row_stats && d.ln_stats), "gemm: a launch either emits LayerNorm statistics or consumes them");
-        l.mode = gemm_fast_mode(d) ? (d.row_stats ? 3 : d.ln_stats ? 4 : 0) : 1;
     }
     if (l.mode != 1 && !(l.mode == 5 && p.trans_first_tile == 0)) {
         // TMA-store boxes of the staged output tile: 64 columns (128-byte swizzle), and a 32-column box (64-byte
@@ -1704,6 +1724,20 @@ extern "C" int64_t pp_gemm_splitk_bytes(const pp_gemm_desc* d0, int32_t* tiles_o
     if (pp::gemm_geometry(d, p, &bn, &ksplit) || ksplit != 2) return 0;
     if (tiles_out) *tiles_out = p.m_tiles * p.n_tiles;
     return (int64_t)p.m_tiles * p.n_tiles * pp::BLOCK_M * bn * 4;
+}
+
+extern "C" pp_status pp_gemm_variant(const pp_gemm_desc* d, int32_t* block_n, int32_t* mode, int32_t* ksplit) {
+    if (!d || !block_n || !mode || !ksplit) {
+        pp::set_last_error("pp_gemm_variant: null argument");
+        return pp::PP_ERR_INVALID;
+    }
+    int bn = 0, m = 0, ks = 0;
+    int rc = pp::gemm_variant(*d, &bn, &m, &ks);
+    if (rc) return rc;
+    *block_n = bn;
+    *mode = m;
+    *ksplit = ks;
+    return pp::PP_OK;
 }
 
 extern "C" pp_status pp_gemm_conv(const pp_gemm_desc* d, pp_stream stream) {

@@ -103,6 +103,7 @@ int attn_launch(const AttnLaunch& l, cudaStream_t s);
 // ---------------------------------------------------------------- simple ops
 int gemm_stats_geometry(const pp_gemm_desc& d, pp_stats_geom* out);
 int gemm_row_stats_records(const pp_gemm_desc& d);
+int gemm_variant(const pp_gemm_desc& d, int* block_n, int* mode, int* ksplit);
 int group_norm_launch(const pp_gn_desc& d, cudaStream_t s);
 int group_norm_validate(const pp_gn_desc& d);
 int64_t group_norm_scratch_bytes(int batch, int hw, int channels, int groups);

@@ -174,6 +174,20 @@ def gemm_row_stats_records(desc: Desc) -> int:
     return int(N.lib().pp_gemm_row_stats_records(C.byref(desc.c)))
 
 
+def gemm_variant(desc: Desc):
+    """host-only: (block_n, mode, ksplit) of the kernel variant pp_gemm_conv would launch for this descriptor"""
+    bn, mode, ks = N.i32(0), N.i32(0), N.i32(0)
+    N.check(N.lib().pp_gemm_variant(C.byref(desc.c), C.byref(bn), C.byref(mode), C.byref(ks)), "pp_gemm_variant")
+    return int(bn.value), int(mode.value), int(ks.value)
+
+
+def attention_variant(desc: Desc):
+    """host-only: (dv, p_fp16) of the kernel variant pp_attention would launch for this descriptor"""
+    dv, f16 = N.i32(0), N.i32(0)
+    N.check(N.lib().pp_attention_variant(C.byref(desc.c), C.byref(dv), C.byref(f16)), "pp_attention_variant")
+    return int(dv.value), int(f16.value)
+
+
 def attach_row_stats(desc: Desc, rec: torch.Tensor, final: torch.Tensor, ticket: torch.Tensor, eps: float) -> None:
     """rec: fp32 scratch [records, ld >= M, 4]; final: fp32 [>= M, 2] receives {rstd, -rstd * mean} per row; ticket: int32
     [>= ceil(M / 128)], zero-initialised (the kernel leaves it at zero)"""
