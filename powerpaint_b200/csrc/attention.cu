@@ -142,14 +142,14 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
             float sc[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) sc[i] = 0.f;
+            // Every wgmma count in this loop is a compile-time constant: a wgmma under a runtime condition makes ptxas
+            // serialise all of them (C7519). Channels d .. DV - 1 of Q and K are TMA zero fill and add exact zeros.
             wgmma_fence();
 #pragma unroll
-            for (int ks = 0; ks < 4 * DCH; ++ks) {
-                if (ks < p.k_steps) {
-                    const int dc = ks >> 2, kk = (ks & 3) * 16;
-                    Wgmma<ATT_BN>::ss_bf16(sc, wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(qa + dc * ATT_CHUNK_BYTES), kk),
-                                           wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(kb + dc * ATT_CHUNK_BYTES), kk), 1);
-                }
+            for (int ks = 0; ks < DV / 16; ++ks) {
+                const int dc = ks >> 2, kk = (ks & 3) * 16;
+                Wgmma<ATT_BN>::ss_bf16(sc, wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(qa + dc * ATT_CHUNK_BYTES), kk),
+                                       wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(kb + dc * ATT_CHUNK_BYTES), kk), 1);
             }
             wgmma_commit();
             wgmma_wait<0>();
@@ -196,16 +196,14 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
                 pa[2 * i] = p01;
                 pa[2 * i + 1] = p23;
             }
-            const int pv_steps = (nvalid + 15) >> 4;  // 16 keys per MMA; 8 unless ragged
+            // all 8 k-steps of 16 keys, ragged block included: keys past the end have P = 0 and V^T = TMA zero fill
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) {
-                if (ks < pv_steps) {
-                    const uint64_t db = wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(vb + (ks >> 2) * V_CHUNK), (ks & 3) * 16);
-                    const uint32_t(&a)[4] = *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * ks]);
-                    if constexpr (F16) Wgmma<DV>::rs_f16(o, a, db, 1);
-                    else Wgmma<DV>::rs_bf16(o, a, db, 1);
-                }
+                const uint64_t db = wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(vb + (ks >> 2) * V_CHUNK), (ks & 3) * 16);
+                const uint32_t(&a)[4] = *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * ks]);
+                if constexpr (F16) Wgmma<DV>::rs_f16(o, a, db, 1);
+                else Wgmma<DV>::rs_bf16(o, a, db, 1);
             }
             wgmma_commit();
             wgmma_wait<0>();
@@ -306,7 +304,6 @@ int attn_prepare(const pp_attn_desc& d, AttnLaunch* out) {
     PP_REQUIRE(d.o_ld >= (int64_t)d.heads * d.d, "attention: o_ld too small");
     PP_REQUIRE((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "attention: out not 16-byte aligned");
     p.batch = d.batch; p.heads = d.heads; p.d = d.d; p.nq = d.nq; p.nk = d.nk;
-    p.k_steps = (d.d + 15) / 16;
     const int dvi = att_dv_index(d.d);
     p.dv = ATT_DVS[dvi];
     p.scale_log2 = d.scale * 1.4426950408889634f;

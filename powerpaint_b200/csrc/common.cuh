@@ -91,21 +91,9 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
     return t;
 }
+// No report before the trap: a printf is a function call, and ptxas serialises every wgmma of a kernel that
+// contains one (warning C7510), whichever warp role the call sits in. The trap surfaces as a launch error.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    if (mbar_try_wait(bar, parity)) return;
-    const uint64_t t0 = global_timer_ns();
-    uint32_t spins = 0;
-    while (!mbar_try_wait(bar, parity)) {
-        if ((++spins & 0xFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) {
-            printf("pp: mbarrier wait timed out (block %d,%d,%d thread %d bar 0x%x parity %u)\n",
-                   blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, bar, parity);
-            __trap();
-        }
-    }
-}
-
-// the same without the report: no function call, so it may sit between asynchronous wgmma operations
-__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const uint64_t t0 = global_timer_ns();
     uint32_t spins = 0;

@@ -381,10 +381,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 uint32_t spins = 0;
                 while (s_req_seq < seq) {
                     __nanosleep(40);
-                    if ((++spins & 0x3FFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) {
-                        printf("pp: ticket server timed out (block %d seq %d)\n", blockIdx.x, seq);
-                        __trap();
-                    }
+                    if ((++spins & 0x3FFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) __trap();
                 }
                 __threadfence_block();
                 const int mt = s_req_mtile;
@@ -499,7 +496,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             for (int i = 0; i < BLOCK_N / 2; ++i) facc[i] = 0.f;
             int prev = 0;
             for (int it = k_begin; it < k_end; ++it) {
-                mbar_wait_quiet(full_bar(ks), kph);  // (a call here would serialise the in-flight MMAs)
+                mbar_wait(full_bar(ks), kph);
                 const uint64_t da = wgmma_desc_kmajor_sw128(sA + ks * A_STAGE_BYTES + wg * (A_STAGE_BYTES / 2));
                 const uint64_t db = wgmma_desc_kmajor_sw128(sB + ks * B_STAGE_BYTES);
                 wgmma_fence();
@@ -522,10 +519,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                     const uint64_t t0 = global_timer_ns();
                     uint32_t spins = 0;
                     while (*fl == 0) {
-                        if ((++spins & 0xFFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) {
-                            printf("pp: split-K owner timed out (block %d)\n", blockIdx.x);
-                            __trap();
-                        }
+                        if ((++spins & 0xFFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) __trap();
                     }
                     __threadfence();
                     *fl = 0;  // ready for the next launch
@@ -596,10 +590,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             const uint64_t t0 = global_timer_ns();
             uint32_t spins = 0;
             while (s_resp_seq < seq) {
-                if ((++spins & 0xFFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) {
-                    printf("pp: ticket verdict timed out (block %d seq %d)\n", blockIdx.x, seq);
-                    __trap();
-                }
+                if ((++spins & 0xFFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) __trap();
             }
             __threadfence_block();
             return s_resp_last;

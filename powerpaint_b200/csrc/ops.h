@@ -84,7 +84,6 @@ int gemm_launch(const GemmLaunch& l, cudaStream_t s);
 struct AttnKParams {
     CUtensorMap tmQ, tmK, tmV;
     int32_t batch, heads, d, nq, nk;
-    int32_t k_steps;   // ceil(d / 16)
     int32_t dv;        // N of the PV product: d rounded up to an instantiated width (>= ceil16(d))
     float scale_log2;  // scale * log2(e)
     int32_t vt_fp16;   // V^T (and P) in fp16 instead of bf16
