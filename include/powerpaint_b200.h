@@ -38,6 +38,8 @@
  *   pp_softmax_rows, pp_image_preprocess_u8, pp_image_postprocess   VAE attention softmax and the uint8
  *                     pre/post-processing either side of vae.encode / vae.decode
  *                     (pipeline_PowerPaint.py:39-153,657-669,1051,1062)
+ *   pp_window_copy, pp_tile_blend   tiled VAE encode / decode (diffusers AutoencoderKL.enable_tiling,
+ *                     pipeline_PowerPaint_ControlNet.py:341-356): tile gather / assembly and the seam blend
  *   pp_embed_gather, pp_causal_attention_small   CLIP text encoder: embeddings with the task-prompt splice
  *                     (utils/utils.py:256-483) and the causal 77-token attention (pipeline_PowerPaint.py:317-518)
  *   pp_program_*      a recorded list of the above, replayed per denoising step (pp_program_run_range: a slice
@@ -281,6 +283,39 @@ pp_status pp_image_preprocess_u8(const uint8_t* image, const void* mask, int32_t
 pp_status pp_image_postprocess(const void* x, int32_t x_is_fp32, int32_t c_ld, uint8_t* out_u8, float* out_f32,
                                int32_t nb, int32_t hw, pp_stream stream);
 
+/* ------------------------------------------------------------------ tiled VAE (diffusers enable_tiling) */
+/* One rectangular window of pixels: `rows` x `cols` pixels starting at element offset src_off of the source and
+   dst_off of the destination, consecutive rows src_row / dst_row elements apart. */
+typedef struct pp_window {
+    int64_t src_off, dst_off;
+    int64_t src_row, dst_row;
+    int32_t rows, cols;
+} pp_window;
+/* Copies `count` windows (a DEVICE array) of `channels` elements per pixel from src to dst, pixels src_pix / dst_pix
+   elements apart; elem_bytes 2 (bf16) or 4 (fp32). max_pixels >= rows * cols of every window sizes the grid.
+   Windows must not overlap in dst. The tiled VAE gathers its tiles out of the canvas with it and assembles the
+   cropped tiles into the output. */
+pp_status pp_window_copy(const void* src, void* dst, int32_t elem_bytes, int32_t channels, int64_t src_pix,
+                         int64_t dst_pix, const pp_window* windows, int32_t count, int32_t max_pixels, pp_stream stream);
+/* In-place blend of one tile b of an fp32 NHWC tile store (`channels` floats per pixel) with the tile above (av)
+   and the tile to its left (ah), for `batch` samples; diffusers AutoencoderKL.blend_v then blend_h:
+     for y < e_v: b[y, :] = av[av_h - e_v + y, :] * (1 - y/e_v) + b[y, :] * (y/e_v)
+     for x < e_h: b[:, x] = ah[:, ah_w - e_h + x] * (1 - x/e_h) + b[:, x] * (x/e_h)
+   Each weight is the double expression rounded to fp32, each product and the sum are rounded separately (no FMA):
+   bit-identical to the torch loop. av has b_w columns and ah has b_h rows; e_v = 0 / e_h = 0 skips a direction
+   (its pointer may then be NULL). Sample s of a tile starts s * *_stride floats after its pointer. */
+typedef struct pp_tile_blend_desc {
+    float* b;
+    const float* av;
+    const float* ah;
+    int64_t b_stride, av_stride, ah_stride;
+    int32_t batch, channels;
+    int32_t b_h, b_w;
+    int32_t av_h, ah_w;
+    int32_t e_v, e_h;
+} pp_tile_blend_desc;
+pp_status pp_tile_blend(const pp_tile_blend_desc* d, pp_stream stream);
+
 /* ------------------------------------------------------------------ text encoder */
 /* out[r] = (idx[r] < vocab ? base[idx[r]] : ext[idx[r] - vocab]) + pos[r % seq]  (bf16 [rows, dim]; fp32 tables).
    CLIP token + position embedding with the EmbeddingLayerWithFixes task-prompt splice (utils.py:256-483) resolved
@@ -385,6 +420,10 @@ pp_status pp_program_add_causal_attention_small(pp_program* p, const void* qkv, 
                                                 int32_t heads, int32_t d, float scale);
 pp_status pp_program_add_softmax_rows(pp_program* p, const float* s, void* out, int64_t rows, int32_t cols,
                                       int64_t ld_s, int64_t ld_p);
+pp_status pp_program_add_window_copy(pp_program* p, const void* src, void* dst, int32_t elem_bytes, int32_t channels,
+                                     int64_t src_pix, int64_t dst_pix, const pp_window* windows, int32_t count,
+                                     int32_t max_pixels);
+pp_status pp_program_add_tile_blend(pp_program* p, const pp_tile_blend_desc* d);
 int32_t pp_program_num_ops(const pp_program* p);
 /* number of kernel launches one run enqueues */
 int32_t pp_program_num_launches(const pp_program* p);

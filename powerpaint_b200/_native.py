@@ -102,6 +102,21 @@ class UniPCDesc(C.Structure):
     ]
 
 
+class Window(C.Structure):
+    _fields_ = [("src_off", i64), ("dst_off", i64), ("src_row", i64), ("dst_row", i64), ("rows", i32), ("cols", i32)]
+
+
+class TileBlendDesc(C.Structure):
+    _fields_ = [
+        ("b", vp), ("av", vp), ("ah", vp),
+        ("b_stride", i64), ("av_stride", i64), ("ah_stride", i64),
+        ("batch", i32), ("channels", i32),
+        ("b_h", i32), ("b_w", i32),
+        ("av_h", i32), ("ah_w", i32),
+        ("e_v", i32), ("e_h", i32),
+    ]
+
+
 # every exported symbol of include/powerpaint_b200.h with (restype, argtypes)
 _SIGNATURES = {
     "pp_last_error": (C.c_char_p, []),
@@ -134,6 +149,10 @@ _SIGNATURES = {
     "pp_image_preprocess_u8": (C.c_int, [vp, vp, i32, vp, i32, i32, i32, f32, f32, vp]),
     "pp_image_postprocess": (C.c_int, [vp, i32, i32, vp, vp, i32, i32, vp]),
     "pp_program_add_softmax_rows": (C.c_int, [vp, vp, vp, i64, i32, i64, i64]),
+    "pp_window_copy": (C.c_int, [vp, vp, i32, i32, i64, i64, vp, i32, i32, vp]),
+    "pp_program_add_window_copy": (C.c_int, [vp, vp, vp, i32, i32, i64, i64, vp, i32, i32]),
+    "pp_tile_blend": (C.c_int, [C.POINTER(TileBlendDesc), vp]),
+    "pp_program_add_tile_blend": (C.c_int, [vp, C.POINTER(TileBlendDesc)]),
     "pp_program_create": (C.c_int, [C.POINTER(vp)]),
     "pp_program_run_range": (C.c_int, [vp, i32, i32, vp]),
     "pp_program_destroy": (None, [vp]),

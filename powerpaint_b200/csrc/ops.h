@@ -120,6 +120,12 @@ int image_preprocess_launch(const uint8_t* img, const void* mask, int mask_mode,
                             float divisor, float shift, cudaStream_t s);
 int image_postprocess_launch(const void* x, int x_fp32, int c_ld, uint8_t* out_u8, float* out_f32, int nb, int hw,
                              cudaStream_t s);
+int window_copy_validate(const void* src, void* dst, int elem_bytes, int channels, int64_t src_pix, int64_t dst_pix,
+                         const pp_window* windows, int count, int max_pixels);
+int window_copy_launch(const void* src, void* dst, int elem_bytes, int channels, int64_t src_pix, int64_t dst_pix,
+                       const pp_window* windows, int count, int max_pixels, cudaStream_t s);
+int tile_blend_validate(const pp_tile_blend_desc& d);
+int tile_blend_launch(const pp_tile_blend_desc& d, cudaStream_t s);
 int embed_gather_launch(const int32_t* idx, const float* base, const float* ext, const float* pos, void* out, int rows,
                         int vocab, int seq, int dim, cudaStream_t s);
 int causal_attention_small_launch(const void* qkv, void* out, int batch, int seq, int heads, int d, float scale,

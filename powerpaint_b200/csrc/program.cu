@@ -16,7 +16,8 @@
 namespace pp {
 
 enum OpKind {
-    OP_GEMM, OP_ATTN, OP_GN, OP_LN, OP_UPSAMPLE, OP_ADD, OP_TIME_EMBED, OP_CFG_DDIM, OP_MEMSET, OP_SOFTMAX, OP_UNIPC, OP_EMBED, OP_CAUSAL_ATTN
+    OP_GEMM, OP_ATTN, OP_GN, OP_LN, OP_UPSAMPLE, OP_ADD, OP_TIME_EMBED, OP_CFG_DDIM, OP_MEMSET, OP_SOFTMAX, OP_UNIPC, OP_EMBED, OP_CAUSAL_ATTN,
+    OP_WINDOW_COPY, OP_TILE_BLEND
 };
 
 struct LnArgs { const void* x; void* y; const float* gamma; const float* beta; int rows, c; float eps; };
@@ -27,6 +28,7 @@ struct MsArgs { void* ptr; int64_t bytes; };
 struct EmArgs { const int32_t* idx; const float* base; const float* ext; const float* pos; void* out; int rows, vocab, seq, dim; };
 struct CaArgs { const void* qkv; void* out; int batch, seq, heads, d; float scale; };
 struct SmArgs { const float* s; void* p; int64_t rows; int cols; int64_t ld_s, ld_p; };
+struct WcArgs { const void* src; void* dst; int elem_bytes, channels; int64_t src_pix, dst_pix; const pp_window* windows; int count, max_pixels; };
 
 struct Op {
     OpKind kind;
@@ -44,6 +46,8 @@ struct Op {
         EmArgs em;
         CaArgs ca;
         pp_unipc_desc unipc;
+        WcArgs wc;
+        pp_tile_blend_desc tb;
     };
     Op() { memset(this, 0, sizeof(*this)); }
 };
@@ -75,6 +79,9 @@ static int run_op(const Op& op, cudaStream_t s) {
         case OP_EMBED: return embed_gather_launch(op.em.idx, op.em.base, op.em.ext, op.em.pos, op.em.out, op.em.rows, op.em.vocab, op.em.seq, op.em.dim, s);
         case OP_CAUSAL_ATTN: return causal_attention_small_launch(op.ca.qkv, op.ca.out, op.ca.batch, op.ca.seq, op.ca.heads, op.ca.d, op.ca.scale, s);
         case OP_SOFTMAX: return softmax_rows_launch(op.sm.s, op.sm.p, op.sm.rows, op.sm.cols, op.sm.ld_s, op.sm.ld_p, s);
+        case OP_WINDOW_COPY: return window_copy_launch(op.wc.src, op.wc.dst, op.wc.elem_bytes, op.wc.channels, op.wc.src_pix,
+                                                       op.wc.dst_pix, op.wc.windows, op.wc.count, op.wc.max_pixels, s);
+        case OP_TILE_BLEND: return tile_blend_launch(op.tb, s);
     }
     set_last_error("program: unknown op kind %d", (int)op.kind);
     return PP_ERR_INVALID;
@@ -273,6 +280,33 @@ pp_status pp_program_add_softmax_rows(pp_program* p, const float* s, void* out, 
     pp::Op op;
     op.kind = pp::OP_SOFTMAX;
     op.sm = {s, out, rows, cols, ld_s, ld_p};
+    p->ops.push_back(op);
+    return pp::PP_OK;
+}
+
+pp_status pp_program_add_window_copy(pp_program* p, const void* src, void* dst, int32_t elem_bytes, int32_t channels,
+                                     int64_t src_pix, int64_t dst_pix, const pp_window* windows, int32_t count,
+                                     int32_t max_pixels) {
+    PP_PROG_CHECK(p);
+    int rc = pp::window_copy_validate(src, dst, elem_bytes, channels, src_pix, dst_pix, windows, count, max_pixels);
+    if (rc) return rc;
+    pp::Op op;
+    op.kind = pp::OP_WINDOW_COPY;
+    op.wc = {src, dst, elem_bytes, channels, src_pix, dst_pix, windows, count, max_pixels};
+    p->ops.push_back(op);
+    return pp::PP_OK;
+}
+
+pp_status pp_program_add_tile_blend(pp_program* p, const pp_tile_blend_desc* d) {
+    PP_PROG_CHECK(p);
+    if (!d) { pp::set_last_error("pp_program_add_tile_blend: null descriptor"); return pp::PP_ERR_INVALID; }
+    int rc = pp::tile_blend_validate(*d);
+    if (rc) return rc;
+    PP_REQUIRE((int64_t)d->e_v * d->b_w + (int64_t)(d->b_h - d->e_v) * d->e_h > 0,
+               "pp_program_add_tile_blend: the tile has no seam to blend");
+    pp::Op op;
+    op.kind = pp::OP_TILE_BLEND;
+    op.tb = *d;
     p->ops.push_back(op);
     return pp::PP_OK;
 }

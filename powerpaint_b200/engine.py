@@ -82,6 +82,7 @@ class Plan:
         self.row_stats: Dict[int, torch.Tensor] = {}   # data_ptr of a tensor -> per-row {rstd, -rstd mean} its producer leaves
         self.row_ticket: Optional[torch.Tensor] = None  # arrival counters of the LayerNorm-statistics producers (kept at zero)
         self.scale_dev: Optional[torch.Tensor] = None  # eager side-net forward: 1-float conditioning scale
+        self.best_fit = False  # recycle the smallest free block at least as large as a request, not only equal ones
 
 
 class NetEngine:
@@ -217,6 +218,9 @@ class NetEngine:
         item = torch.empty(0, dtype=dtype).element_size()
         nbytes = (numel * item + 255) // 256 * 256
         pool = plan.free.get(nbytes)
+        if not pool and plan.best_fit:
+            fits = [n for n, blocks in plan.free.items() if blocks and n > nbytes]
+            pool = plan.free[min(fits)] if fits else None
         if pool:
             raw = pool.pop()
         else:

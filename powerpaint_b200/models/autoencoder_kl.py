@@ -25,8 +25,9 @@ from __future__ import annotations
 
 import math
 from collections import OrderedDict
+from dataclasses import dataclass
 from types import SimpleNamespace
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -99,6 +100,88 @@ def vae_param_shapes(in_channels=3, out_channels=3, latent_channels=4, block_out
     return d
 
 
+# --------------------------------------------------------------------------- tile geometry
+# Attention S = QK^T of one image is a [hw, hw] fp32 matrix and pp_softmax_rows takes at most 16384 columns
+VAE_MAX_LATENT_PIXELS = 16384
+
+
+@dataclass(frozen=True)
+class VaeTile:
+    """One tile of diffusers' tiled_encode / tiled_decode loop (row-major order)."""
+    row: int
+    col: int
+    y: int        # origin in the input (image for encode, latent for decode)
+    x: int
+    h: int        # input extent: the tile slice is clipped at the input's border
+    w: int
+    out_h: int    # extent of the encoded / decoded tile
+    out_w: int
+    crop_h: int   # the tile's top-left crop that lands in the output
+    crop_w: int
+    dst_y: int    # where the crop lands
+    dst_x: int
+    blend_v: int  # rows blended with the tile above (0: none)
+    blend_h: int  # columns blended with the tile to the left (0: none)
+
+
+@dataclass(frozen=True)
+class VaeTileGeometry:
+    rows: int
+    cols: int
+    out_h: int
+    out_w: int
+    tiles: Tuple[VaeTile, ...]
+
+    def groups(self) -> "OrderedDict[Tuple[int, int], List[int]]":
+        """tile indices per input shape (h, w), in row-major order of first appearance"""
+        g: "OrderedDict[Tuple[int, int], List[int]]" = OrderedDict()
+        for k, t in enumerate(self.tiles):
+            g.setdefault((t.h, t.w), []).append(k)
+        return g
+
+
+def vae_tile_geometry(encode: bool, h: int, w: int, tile_sample_min_size: int, tile_latent_min_size: int,
+                      tile_overlap_factor: float, scale: int) -> VaeTileGeometry:
+    """The tiles of diffusers 0.27 `AutoencoderKL.tiled_encode` (image h x w) or `tiled_decode` (latent h x w):
+    origins every int(tile * (1 - f)) input pixels, blend extent int(out_tile * f), crop to out_tile - extent.
+    `scale` = 2 ** (len(block_out_channels) - 1): a decoded tile is `scale` times its latent, an encoded tile is
+    its image floor-divided by 2 once per downsampler."""
+    f = tile_overlap_factor
+    if encode:
+        tin, tout = tile_sample_min_size, tile_latent_min_size
+
+        def out_size(n):
+            return n // scale
+    else:
+        tin, tout = tile_latent_min_size, tile_sample_min_size
+
+        def out_size(n):
+            return n * scale
+    overlap = int(tin * (1 - f))
+    blend = int(tout * f)
+    limit = tout - blend
+    if overlap <= 0:
+        raise ValueError(f"tile size {tin} with overlap factor {f} gives no tile stride")
+    ys, xs = list(range(0, h, overlap)), list(range(0, w, overlap))
+    tiles = []
+    dst_y = 0
+    for r, y in enumerate(ys):
+        th = min(tin, h - y)
+        oh = out_size(th)
+        ch = len(range(oh)[:limit])  # tile[:limit] in Python slice semantics
+        dst_x = 0
+        for c, x in enumerate(xs):
+            tw = min(tin, w - x)
+            ow = out_size(tw)
+            cw = len(range(ow)[:limit])
+            ev = min(out_size(min(tin, h - ys[r - 1])), oh, blend) if r > 0 else 0
+            eh = min(out_size(min(tin, w - xs[c - 1])), ow, blend) if c > 0 else 0
+            tiles.append(VaeTile(r, c, y, x, th, tw, oh, ow, ch, cw, dst_y, dst_x, max(ev, 0), max(eh, 0)))
+            dst_x += cw
+        dst_y += ch
+    return VaeTileGeometry(len(ys), len(xs), dst_y, dst_x, tuple(tiles))
+
+
 # --------------------------------------------------------------------------- engine
 class VaeEngine(NetEngine):
     """Records VAE encode / decode as `pp_program`s over the conv / GroupNorm / GEMM kernels of the denoising
@@ -147,11 +230,14 @@ class VaeEngine(NetEngine):
         bqk = self._cached("vqkb:" + name, lambda: torch.cat(
             [self._raw(name + ".to_q.bias"), self._raw(name + ".to_k.bias")], 0).contiguous())
         qk = self._linear(plan, prog, g, M, None, 2 * C, w=wqk, bias=bqk)
-        # V^T [nb, C, hw_ld] and P [hw, hw_ld]: zero-initialised once, the kernels never write the pad columns
-        vt = torch.zeros(nb, C, hw_ld, dtype=BF16, device=self.device)
-        pm = torch.zeros(hw, hw_ld, dtype=BF16, device=self.device)
-        sm = torch.empty(hw, hw, dtype=torch.float32, device=self.device)
-        plan.bytes += vt.numel() * 2 + pm.numel() * 2 + sm.numel() * 4
+        # V^T [nb, C, hw_ld] and P [hw, hw_ld]: the kernels never write the pad columns, which the PV product reads,
+        # so a recycled block is cleared first
+        vt = self._buf(plan, nb, C, hw_ld)
+        pm = self._buf(plan, hw, hw_ld)
+        if hw_ld != hw:
+            prog.add_memset(vt)
+            prog.add_memset(pm)
+        sm = self._buf(plan, hw, hw, dtype=torch.float32)
         prog.add(ops.gemm_desc(a0=g, w=self.w_linear(name + ".to_v"), out=vt, N_=C, M=M, bias=self.vec(name + ".to_v.bias"),
                                epilogue=N.PP_EPI_TRANSPOSED, t_rows=hw, t_ld=hw_ld))
         self._free(plan, g)
@@ -163,7 +249,7 @@ class VaeEngine(NetEngine):
                                    out_fp32=True))
             prog.add_softmax_rows(sm, pm, hw, hw, hw, hw_ld)
             prog.add(ops.gemm_desc(a0=pm, c0=hw_ld, lda0=hw_ld, w=vt[b], ldb=hw_ld, out=o[b * hw:(b + 1) * hw], N_=C, M=hw))
-        self._free(plan, qk)
+        self._free(plan, qk, vt, pm, sm)
         out = self._linear(plan, prog, o, M, name + ".to_out.0", C, bias=self.vec(name + ".to_out.0.bias"), res1=x,
                            stats_hw=hw)
         self._free(plan, o)
@@ -189,17 +275,37 @@ class VaeEngine(NetEngine):
         self._plans[key] = p
         return p
 
+    def _check_latent(self, h: int, w: int, what: str):
+        if h * w > VAE_MAX_LATENT_PIXELS:
+            raise RuntimeError(
+                f"VAE {what}: a {h}x{w} latent has {h * w} pixels, above the {VAE_MAX_LATENT_PIXELS} the VAE's "
+                "mid-block attention supports per image (1048576 image pixels); call enable_vae_tiling() "
+                "(AutoencoderKL.enable_tiling()) to encode / decode larger images tile by tile")
+
+    def _latent_hw(self, H: int, W: int):
+        for _ in range(len(self.cfg.block_out_channels) - 1):
+            H, W = H // 2, W // 2
+        return H, W
+
     # ---- encoder
     def encode_plan(self, nb: int, H: int, W: int) -> Plan:
+        self._check_latent(*self._latent_hw(H, W), "encode")
         return self._get_plan(("enc", nb, H, W), lambda: self._build_encode(nb, H, W))
 
-    def _build_encode(self, nb, H, W) -> Plan:
+    def _build_encode(self, nb, H, W, plan: Optional[Plan] = None, x_in: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None) -> Plan:
+        """records the encoder into `plan` (a new one by default), reading bf16 NHWC x_in [nb, H*W, 8] and writing
+        the fp32 moments [nb, h*w, 2 * latent_channels] to `out`"""
         cfg = self.cfg
         boc = cfg.block_out_channels
-        plan = Plan()
-        prog = plan.program = ops.Program()
-        x_in = torch.zeros(nb, H * W, 8, dtype=BF16, device=self.device)
-        plan.inputs["x"] = x_in
+        self._check_latent(*self._latent_hw(H, W), "encode")
+        if plan is None:
+            plan = Plan()
+            plan.program = ops.Program()
+        prog = plan.program
+        if x_in is None:
+            x_in = torch.zeros(nb, H * W, 8, dtype=BF16, device=self.device)
+            plan.inputs["x"] = x_in
         h, w = H, W
         cur = self._conv3(plan, prog, x_in, nb, h, w, "encoder.conv_in", boc[0], pad_in=8, stats=True)
         for i, co in enumerate(boc):
@@ -228,26 +334,35 @@ class VaeEngine(NetEngine):
             bf = wq @ self._raw("encoder.conv_out.bias") + self._raw("quant_conv.bias")
             return ops.pack_conv3x3_weight(wf), bf.contiguous()
         wf, bf = self._cached("enc_out_folded", folded)
-        moments = torch.empty(nb, h * w, lc2, dtype=torch.float32, device=self.device)
+        moments = out if out is not None else torch.empty(nb, h * w, lc2, dtype=torch.float32, device=self.device)
         prog.add(ops.gemm_desc(a0=gno, w=wf, out=moments, N_=lc2, a_mode=N.PP_A_CONV3X3, c0=gno.shape[-1], nb=nb, h=h,
                                w_=w, bias=bf, out_fp32=True))
         self._free(plan, gno)
-        plan.outputs["moments"] = moments
-        plan.outputs["hw"] = (h, w)
+        if out is None:
+            plan.outputs["moments"] = moments
+            plan.outputs["hw"] = (h, w)
         return plan
 
     # ---- decoder
     def decode_plan(self, nb: int, h: int, w: int) -> Plan:
+        self._check_latent(h, w, "decode")
         return self._get_plan(("dec", nb, h, w), lambda: self._build_decode(nb, h, w))
 
-    def _build_decode(self, nb, h, w) -> Plan:
+    def _build_decode(self, nb, h, w, plan: Optional[Plan] = None, z_in: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None) -> Plan:
+        """records the decoder into `plan` (a new one by default), reading bf16 NHWC z_in [nb, h*w, 8] and writing
+        the fp32 image [nb, H*W, 4] (channels 0..2) to `out`"""
         cfg = self.cfg
         rev = list(reversed(cfg.block_out_channels))
         lc = cfg.latent_channels
-        plan = Plan()
-        prog = plan.program = ops.Program()
-        z_in = torch.zeros(nb, h * w, 8, dtype=BF16, device=self.device)
-        plan.inputs["z"] = z_in
+        self._check_latent(h, w, "decode")
+        if plan is None:
+            plan = Plan()
+            plan.program = ops.Program()
+        prog = plan.program
+        if z_in is None:
+            z_in = torch.zeros(nb, h * w, 8, dtype=BF16, device=self.device)
+            plan.inputs["z"] = z_in
         # post_quant_conv (1x1, latent -> latent): its own GEMM; channels >= lc of the output stay zero
         zq = torch.zeros(nb, h * w, 8, dtype=BF16, device=self.device)
         wpq = self._cached("pq:w", lambda: torch.nn.functional.pad(
@@ -270,13 +385,82 @@ class VaeEngine(NetEngine):
         gno = self._gn(plan, prog, cur, None, nb, h * w, "decoder.conv_norm_out", self.GN_EPS, True)
         self._free(plan, cur)
         # fp32 image, 4 floats per pixel (3 used): the uint8 conversion must not see a bf16-rounded value
-        image = torch.zeros(nb, h * w, 4, dtype=torch.float32, device=self.device)
+        image = out if out is not None else torch.zeros(nb, h * w, 4, dtype=torch.float32, device=self.device)
         prog.add(ops.gemm_desc(a0=gno, w=self.w_conv3("decoder.conv_out"), out=image, N_=cfg.out_channels,
                                a_mode=N.PP_A_CONV3X3, c0=gno.shape[-1], nb=nb, h=h, w_=w,
                                bias=self.vec("decoder.conv_out.bias"), out_fp32=True, ldc=4))
         self._free(plan, gno)
-        plan.outputs["image"] = image
-        plan.outputs["hw"] = (h, w)
+        if out is None:
+            plan.outputs["image"] = image
+            plan.outputs["hw"] = (h, w)
+        return plan
+
+    # ---- tiled encode / decode
+    # image pixels one recorded encoder / decoder pass covers (four 512^2 tiles, the pixels of one 1024^2 image):
+    # the activation pool of a tiled plan is sized by one such pass, whatever the canvas
+    TILE_CHUNK_PIXELS = 4 * 512 * 512
+
+    def tiled_plan(self, encode: bool, nb: int, H: int, W: int, geom: VaeTileGeometry, key: tuple) -> Plan:
+        return self._get_plan(("tenc" if encode else "tdec", nb, H, W) + key,
+                              lambda: self._build_tiled(encode, nb, H, W, geom))
+
+    def _restart_gn_arena(self, plan, prog):
+        """the next GroupNorms start over at the head of the current arena, cleared again at this point"""
+        ent = plan.gn_arenas.get(id(prog))
+        if ent is not None and ent[1]:
+            prog.add_memset(ent[0])
+            ent[1] = 0
+
+    def _build_tiled(self, encode: bool, nb: int, H: int, W: int, geom: VaeTileGeometry) -> Plan:
+        """ONE program over the whole canvas: per tile shape, gather the tiles of every sample out of the canvas and
+        run the encoder / decoder on them in chunks of TILE_CHUNK_PIXELS, each writing its slab of an fp32 tile
+        store; then blend every tile with its upper and left neighbours in diffusers' row-major order, in place;
+        then copy each tile's crop into the output. Every chunk records into the plan's one activation pool."""
+        cfg = self.cfg
+        plan = Plan()
+        plan.best_fit = True
+        prog = plan.program = ops.Program()
+        C = 2 * cfg.latent_channels if encode else 4
+        canvas = torch.zeros(nb, H * W, 8, dtype=BF16, device=self.device)
+        out = torch.zeros(nb, geom.out_h * geom.out_w, C, dtype=torch.float32, device=self.device)
+        plan.bytes += canvas.numel() * 2 + out.numel() * 4
+        plan.inputs["x" if encode else "z"] = canvas
+        build = self._build_encode if encode else self._build_decode
+        views: Dict[int, torch.Tensor] = {}  # tile -> fp32 [nb, out_h, out_w, C] in its group's store
+        assembly = []
+        # largest tiles first: with best-fit recycling the smaller passes that follow reuse their blocks
+        for (th, tw), idx in sorted(geom.groups().items(), key=lambda g: -g[0][0] * g[0][1]):
+            t0 = geom.tiles[idx[0]]
+            ohw = t0.out_h * t0.out_w
+            store = torch.zeros(len(idx) * nb, ohw, C, dtype=torch.float32, device=self.device)
+            plan.bytes += store.numel() * 4
+            images = [(k, s) for k in idx for s in range(nb)]  # row r of the store holds images[r]
+            per = max(1, self.TILE_CHUNK_PIXELS // (th * tw if encode else ohw))
+            for r0 in range(0, len(images), per):
+                chunk = images[r0:r0 + per]
+                x_in = self._buf(plan, len(chunk), th * tw, 8)
+                gather = [((s * H * W + geom.tiles[k].y * W + geom.tiles[k].x) * 8, m * th * tw * 8, W * 8, tw * 8,
+                           th, tw) for m, (k, s) in enumerate(chunk)]
+                prog.add_window_copy(ops.WindowList(canvas, x_in, 8, gather))
+                self._restart_gn_arena(plan, prog)
+                build(len(chunk), th, tw, plan, x_in, store[r0:r0 + len(chunk)])
+                self._free(plan, x_in)
+            crops = []
+            for j, k in enumerate(idx):
+                t = geom.tiles[k]
+                views[k] = store[j * nb:(j + 1) * nb].view(nb, t.out_h, t.out_w, C)
+                crops += [((j * nb + s) * ohw * C, (s * geom.out_h * geom.out_w + t.dst_y * geom.out_w + t.dst_x) * C,
+                           t.out_w * C, geom.out_w * C, t.crop_h, t.crop_w) for s in range(nb)]
+            if any(c[4] and c[5] for c in crops):
+                assembly.append(ops.WindowList(store, out, C, crops))
+        for k, t in enumerate(geom.tiles):
+            if t.blend_v or t.blend_h:
+                prog.add(ops.tile_blend_desc(views[k], views[k - geom.cols] if t.blend_v else None,
+                                             views[k - 1] if t.blend_h else None, t.blend_v, t.blend_h))
+        for wl in assembly:
+            prog.add_window_copy(wl)
+        plan.outputs["moments" if encode else "image"] = out
+        plan.outputs["hw"] = (geom.out_h, geom.out_w)
         return plan
 
 
@@ -299,7 +483,7 @@ class DiagonalGaussianDistribution:
 class AutoencoderKL(nn.Module):
     def __init__(self, in_channels: int = 3, out_channels: int = 3, latent_channels: int = 4,
                  block_out_channels: Tuple[int, ...] = (128, 256, 512, 512), layers_per_block: int = 2,
-                 norm_num_groups: int = 32, scaling_factor: float = 0.18215):
+                 norm_num_groups: int = 32, scaling_factor: float = 0.18215, sample_size: int = 32):
         super().__init__()
         if in_channels != 3 or out_channels != 3 or latent_channels > 4:
             raise NotImplementedError("the kernel path is built for RGB images and <= 4 latent channels (SD VAE)")
@@ -308,7 +492,14 @@ class AutoencoderKL(nn.Module):
         self.config = SimpleNamespace(in_channels=in_channels, out_channels=out_channels,
                                       latent_channels=latent_channels, block_out_channels=tuple(block_out_channels),
                                       layers_per_block=layers_per_block, scaling_factor=scaling_factor,
-                                      norm_num_groups=norm_num_groups)
+                                      norm_num_groups=norm_num_groups, sample_size=sample_size)
+        # tiled encode / decode, off by default (diffusers AutoencoderKL.__init__); the tile_* attributes may be set
+        self.use_tiling = False
+        self.use_slicing = False
+        self.tile_sample_min_size = sample_size
+        ss = sample_size[0] if isinstance(sample_size, (list, tuple)) else sample_size
+        self.tile_latent_min_size = int(ss / (2 ** (len(block_out_channels) - 1)))
+        self.tile_overlap_factor = 0.25
         for name, shape in vae_param_shapes(in_channels, out_channels, latent_channels, block_out_channels,
                                             layers_per_block).items():
             self._register(name, torch.zeros(shape))
@@ -363,40 +554,79 @@ class AutoencoderKL(nn.Module):
             self._engine = VaeEngine(self.config, {k: v for k, v in self.state_dict().items()}, dev)
         return self._engine
 
+    # ---- tiling (diffusers AutoencoderKL.enable_tiling: opt-in, it blends tile seams and so changes the result)
+    def enable_tiling(self, use_tiling: bool = True):
+        """encode / decode images above tile_sample_min_size (latents above tile_latent_min_size) tile by tile"""
+        self.use_tiling = use_tiling
+
+    def disable_tiling(self):
+        self.enable_tiling(False)
+
+    def tile_geometry(self, encode: bool, h: int, w: int) -> VaeTileGeometry:
+        """the tiles tiled_encode (image h x w) / tiled_decode (latent h x w) runs with the current tile_* settings"""
+        return vae_tile_geometry(encode, h, w, self.tile_sample_min_size, self.tile_latent_min_size,
+                                 self.tile_overlap_factor, 2 ** (len(self.config.block_out_channels) - 1))
+
+    def _tiling_key(self):
+        return (self.tile_sample_min_size, self.tile_latent_min_size, self.tile_overlap_factor)
+
     # ---- encode
     @torch.no_grad()
-    def _moments(self, x_nhwc: torch.Tensor, nb: int, H: int, W: int) -> torch.Tensor:
-        plan = self.engine().encode_plan(nb, H, W)
+    def _moments(self, x_nhwc: torch.Tensor, nb: int, H: int, W: int, tiled: bool = False) -> torch.Tensor:
+        eng = self.engine()
+        if tiled:
+            plan = eng.tiled_plan(True, nb, H, W, self.tile_geometry(True, H, W), self._tiling_key())
+        else:
+            plan = eng.encode_plan(nb, H, W)
         plan.inputs["x"].copy_(x_nhwc.view_as(plan.inputs["x"]))
         plan.program.launch()
         h, w = plan.outputs["hw"]
         return ops.nhwc_to_nchw(plan.outputs["moments"].view(nb, h, w, -1)).to(self._out_dtype)
 
+    def _tile_image(self, H: int, W: int) -> bool:
+        return self.use_tiling and (W > self.tile_sample_min_size or H > self.tile_sample_min_size)
+
+    def _tile_latent(self, h: int, w: int) -> bool:
+        return self.use_tiling and (w > self.tile_latent_min_size or h > self.tile_latent_min_size)
+
     @torch.no_grad()
-    def encode(self, x: torch.Tensor, return_dict: bool = True):
-        """x [B,3,H,W] in [-1,1] -> `.latent_dist` (DiagonalGaussianDistribution over [B,8,H/8,W/8] moments)"""
+    def _encode(self, x: torch.Tensor, return_dict: bool, tiled: bool):
         nb, c, H, W = x.shape
         self.engine()  # raises on CPU parameters: there is no CPU path
         with torch.cuda.device(self.device):
             xn = ops.nchw_to_nhwc(x.to(self.device).float().contiguous(), 8)
-            dist = DiagonalGaussianDistribution(self._moments(xn, nb, H, W))
+            dist = DiagonalGaussianDistribution(self._moments(xn, nb, H, W, tiled))
         return SimpleNamespace(latent_dist=dist) if return_dict else (dist,)
+
+    def encode(self, x: torch.Tensor, return_dict: bool = True):
+        """x [B,3,H,W] in [-1,1] -> `.latent_dist` (DiagonalGaussianDistribution over [B,8,H/8,W/8] moments);
+        tiled (`tiled_encode`) when tiling is on and a side exceeds tile_sample_min_size"""
+        return self._encode(x, return_dict, self._tile_image(x.shape[-2], x.shape[-1]))
+
+    def tiled_encode(self, x: torch.Tensor, return_dict: bool = True):
+        """diffusers tiled_encode: overlapping tiles through the encoder, their moments blended at the seams"""
+        return self._encode(x, return_dict, True)
 
     @torch.no_grad()
     def encode_uint8(self, image_u8: torch.Tensor, mask: Optional[torch.Tensor] = None) -> DiagonalGaussianDistribution:
         """uint8 NCHW image (hole zeroed where mask >= 0.5) straight into the encoder: `image / 127.5 - 1`,
-        binarise, `image * (mask < 0.5)` (pipeline_PowerPaint.py:123-147) and the layout change are one kernel"""
+        binarise, `image * (mask < 0.5)` (pipeline_PowerPaint.py:123-147) and the layout change are one kernel
+        (over the whole canvas; a tiled encode gathers its tiles from its output)"""
         nb, c, H, W = image_u8.shape
         self.engine()
         with torch.cuda.device(self.device):
             xn = ops.image_preprocess_u8(image_u8.contiguous(), mask, c_pad=8)
-            return DiagonalGaussianDistribution(self._moments(xn, nb, H, W))
+            return DiagonalGaussianDistribution(self._moments(xn, nb, H, W, self._tile_image(H, W)))
 
     # ---- decode
     @torch.no_grad()
-    def _decode_nhwc(self, z: torch.Tensor):
+    def _decode_nhwc(self, z: torch.Tensor, tiled: bool):
         nb, c, h, w = z.shape
-        plan = self.engine().decode_plan(nb, h, w)
+        eng = self.engine()
+        if tiled:
+            plan = eng.tiled_plan(False, nb, h, w, self.tile_geometry(False, h, w), self._tiling_key())
+        else:
+            plan = eng.decode_plan(nb, h, w)
         zi = plan.inputs["z"]
         zi.copy_(ops.nchw_to_nhwc(z.to(self.device).float().contiguous(), 8).view_as(zi))
         plan.program.launch()
@@ -404,20 +634,29 @@ class AutoencoderKL(nn.Module):
         return plan.outputs["image"], nb, H, W
 
     @torch.no_grad()
-    def decode(self, z: torch.Tensor, return_dict: bool = True, generator=None):
+    def _decode(self, z: torch.Tensor, return_dict: bool, tiled: bool):
         self.engine()
         with torch.cuda.device(self.device):
-            img, nb, H, W = self._decode_nhwc(z)
+            img, nb, H, W = self._decode_nhwc(z, tiled)
             out = ops.nhwc_to_nchw(img.view(nb, H, W, 4), 3).to(self._out_dtype)
         return SimpleNamespace(sample=out) if return_dict else (out,)
+
+    def decode(self, z: torch.Tensor, return_dict: bool = True, generator=None):
+        """tiled (`tiled_decode`) when tiling is on and a latent side exceeds tile_latent_min_size"""
+        return self._decode(z, return_dict, self._tile_latent(z.shape[-2], z.shape[-1]))
+
+    def tiled_decode(self, z: torch.Tensor, return_dict: bool = True):
+        """diffusers tiled_decode: overlapping latent tiles through the decoder, blended at the seams"""
+        return self._decode(z, return_dict, True)
 
     @torch.no_grad()
     def decode_postprocessed(self, z: torch.Tensor, uint8: bool) -> torch.Tensor:
         """decode + `VaeImageProcessor.postprocess` denormalisation in one pass over the image:
-        uint8 NHWC [B,H,W,3] (what "pil" output is built from) or fp32 NCHW in [0,1] ("pt" / "np")"""
+        uint8 NHWC [B,H,W,3] (what "pil" output is built from) or fp32 NCHW in [0,1] ("pt" / "np");
+        tiled like `decode`"""
         self.engine()
         with torch.cuda.device(self.device):
-            img, nb, H, W = self._decode_nhwc(z)
+            img, nb, H, W = self._decode_nhwc(z, self._tile_latent(z.shape[-2], z.shape[-1]))
             return ops.image_postprocess(img, nb, H, W, uint8=uint8)
 
     # ---- checkpoint directories in the diffusers layout (`<root>/vae`)
@@ -426,7 +665,7 @@ class AutoencoderKL(nn.Module):
         if config.get("act_fn", "silu") != "silu":
             raise NotImplementedError(f"config.act_fn = {config['act_fn']!r}: the SD VAE uses silu")
         keys = ("in_channels", "out_channels", "latent_channels", "block_out_channels", "layers_per_block",
-                "norm_num_groups", "scaling_factor")
+                "norm_num_groups", "scaling_factor", "sample_size")
         return cls(**{k: (tuple(config[k]) if isinstance(config[k], list) else config[k]) for k in keys if k in config})
 
     @classmethod

@@ -282,7 +282,74 @@ def unipc_desc(*, eps, eps_fp32, eps_ld, latents, last_sample, m1, m2, coef, uco
     return Desc("unipc", d, (eps, latents, last_sample, m1, m2, coef, ucoef, step_idx, next_in))
 
 
+def _tile_view(t: torch.Tensor, name: str):
+    """fp32 [batch, h, w, channels] with every sample contiguous (samples may sit any stride apart)"""
+    if t.dtype != torch.float32 or t.dim() != 4 or not t.is_cuda:
+        raise ValueError(f"{name} must be a CUDA fp32 [batch, h, w, channels] tensor")
+    _, h, w, c = t.shape
+    if t.stride()[1:] != (w * c, c, 1):
+        raise ValueError(f"{name}: each sample must be contiguous")
+    return t.shape
+
+
+def tile_blend_desc(b: torch.Tensor, av: Optional[torch.Tensor], ah: Optional[torch.Tensor], e_v: int,
+                    e_h: int) -> Desc:
+    """In-place blend_v (with av, the tile above, over e_v rows) then blend_h (with ah, the tile to the left, over
+    e_h columns) of the fp32 tile b [batch, h, w, channels] (include/powerpaint_b200.h, pp_tile_blend_desc)"""
+    nb, bh, bw, c = _tile_view(b, "b")
+    d = N.TileBlendDesc()
+    d.b, d.b_stride, d.batch, d.channels, d.b_h, d.b_w = N.ptr(b), b.stride(0), nb, c, bh, bw
+    d.e_v, d.e_h = e_v, e_h
+    if e_v:
+        s = _tile_view(av, "av")
+        if (s[0], s[2], s[3]) != (nb, bw, c):
+            raise ValueError(f"av {tuple(s)} does not sit above b {tuple(b.shape)}")
+        d.av, d.av_stride, d.av_h = N.ptr(av), av.stride(0), s[1]
+    if e_h:
+        s = _tile_view(ah, "ah")
+        if (s[0], s[1], s[3]) != (nb, bh, c):
+            raise ValueError(f"ah {tuple(s)} does not sit left of b {tuple(b.shape)}")
+        d.ah, d.ah_stride, d.ah_w = N.ptr(ah), ah.stride(0), s[2]
+    return Desc("tile_blend", d, (b, av, ah))
+
+
+class WindowList:
+    """Windows (src_off, dst_off, src_row, dst_row, rows, cols) in elements of src / dst, checked against both
+    tensors on the host and uploaded once; `channels` elements are copied per pixel, pixels src_pix / dst_pix
+    elements apart (pp_window_copy)."""
+
+    def __init__(self, src: torch.Tensor, dst: torch.Tensor, channels: int, windows, src_pix: Optional[int] = None,
+                 dst_pix: Optional[int] = None):
+        if src.dtype != dst.dtype or src.dtype not in (BF16, torch.float32):
+            raise TypeError("window copy: src and dst must both be bf16 or both fp32")
+        if not (src.is_cuda and dst.is_cuda and src.is_contiguous() and dst.is_contiguous()):
+            raise ValueError("window copy: src and dst must be contiguous CUDA tensors")
+        self.src_pix = src_pix or src.shape[-1]
+        self.dst_pix = dst_pix or dst.shape[-1]
+        windows = [tuple(int(v) for v in w) for w in windows if w[4] > 0 and w[5] > 0]
+        if not windows:
+            raise ValueError("window copy: no non-empty window")
+        for so, do, sr, dr, rows, cols in windows:
+            for off, row, pix, n, what in ((so, sr, self.src_pix, src.numel(), "src"),
+                                           (do, dr, self.dst_pix, dst.numel(), "dst")):
+                if off < 0 or row < 0 or off + (rows - 1) * row + (cols - 1) * pix + channels > n:
+                    raise ValueError(f"window copy: window {(so, do, sr, dr, rows, cols)} leaves {what}")
+        arr = (N.Window * len(windows))(*[N.Window(*w) for w in windows])
+        self.table = torch.frombuffer(bytearray(arr), dtype=torch.uint8).to(src.device)
+        self.src, self.dst, self.channels = src, dst, channels
+        self.count = len(windows)
+        self.max_pixels = max(w[4] * w[5] for w in windows)
+
+    def args(self):
+        return (N.ptr(self.src), N.ptr(self.dst), self.src.element_size(), self.channels, self.src_pix, self.dst_pix,
+                N.ptr(self.table), self.count, self.max_pixels)
+
+
 # --------------------------------------------------------------------------- immediate mode
+def window_copy(wl: WindowList) -> None:
+    N.check(N.lib().pp_window_copy(*wl.args(), N.current_stream()), "pp_window_copy")
+
+
 def run(desc: Desc) -> None:
     L = N.lib()
     s = N.current_stream()
@@ -296,6 +363,8 @@ def run(desc: Desc) -> None:
         N.check(L.pp_cfg_ddim_step(C.byref(desc.c), s), "pp_cfg_ddim_step")
     elif desc.kind == "unipc":
         N.check(L.pp_unipc_step(C.byref(desc.c), s), "pp_unipc_step")
+    elif desc.kind == "tile_blend":
+        N.check(L.pp_tile_blend(C.byref(desc.c), s), "pp_tile_blend")
     else:
         raise ValueError(desc.kind)
 
@@ -424,7 +493,7 @@ class Program:
         L = N.lib()
         fn = {"gemm": L.pp_program_add_gemm, "attn": L.pp_program_add_attention,
               "gn": L.pp_program_add_group_norm, "cfg_ddim": L.pp_program_add_cfg_ddim,
-              "unipc": L.pp_program_add_unipc}[desc.kind]
+              "unipc": L.pp_program_add_unipc, "tile_blend": L.pp_program_add_tile_blend}[desc.kind]
         N.check(fn(self._h, C.byref(desc.c)), f"pp_program_add_{desc.kind}")
         self._keep.append(desc.keep)
         self.labels.append(desc.kind)
@@ -452,6 +521,11 @@ class Program:
                 "pp_program_add_softmax_rows")
         self._keep.append((s, p))
         self.labels.append("softmax_rows")
+
+    def add_window_copy(self, wl: WindowList):
+        N.check(N.lib().pp_program_add_window_copy(self._h, *wl.args()), "pp_program_add_window_copy")
+        self._keep.append(wl)
+        self.labels.append("window_copy")
 
     def add_embed_gather(self, idx, base, ext, pos, out, rows, vocab, seq, dim):
         N.check(N.lib().pp_program_add_embed_gather(self._h, N.ptr(idx), N.ptr(base), N.ptr(ext), N.ptr(pos), N.ptr(out),

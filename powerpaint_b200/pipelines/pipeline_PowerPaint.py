@@ -318,10 +318,12 @@ class StableDiffusionInpaintPipeline:
         pass
 
     def enable_vae_tiling(self):
-        raise NotImplementedError("tiled VAE decoding (it blends tile borders, i.e. changes the result) is not built")
+        """encode / decode through overlapping VAE tiles blended at the seams (ref:…ControlNet.py:341-356): images
+        above 1024 x 1024 pixels then fit, at the price of a result that differs from the untiled one at the seams"""
+        self.vae.enable_tiling()
 
     def disable_vae_tiling(self):
-        pass
+        self.vae.disable_tiling()
 
     def prepare_mask_latents(self, mask, masked_image, batch_size, height, width, dtype, device, generator,
                              do_classifier_free_guidance):
