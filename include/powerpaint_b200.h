@@ -27,6 +27,8 @@
  *                     (pipelines/pipeline_PowerPaint.py:990-996,1018-1023;
  *                      pipeline_PowerPaint_Brushnet_CA.py:1390,1444-1449)
  *   pp_unipc_step     CFG combine + UniPCMultistepScheduler.step (the v2 app's scheduler, app.py:197)
+ *   pp_solver_step    CFG combine + DPMSolverMultistepScheduler / EulerDiscreteScheduler /
+ *                     EulerAncestralDiscreteScheduler.step (the scheduler a user swaps in, as app.py:197 does)
  *   pp_upsample_nearest  Upsample2D with an explicit output size (unet_2d_condition.py:1120-1126,1311-1312)
  *                     Also carries: LayerNorm of BasicTransformerBlock folded into the producing / consuming
  *                     GEMMs (row_stats / ln_stats; diffusers LayerNorm norm1/2/3, SURVEY.md App. A.3), and
@@ -393,6 +395,33 @@ typedef struct pp_unipc_desc {
 } pp_unipc_desc;
 pp_status pp_unipc_step(const pp_unipc_desc* d, pp_stream stream);
 
+/* CFG combine + one step of DPMSolverMultistepScheduler (dpmsolver++ / sde-dpmsolver++, solver_order 1 or 2),
+   EulerDiscreteScheduler or EulerAncestralDiscreteScheduler + next-step input build. Each update is linear in the
+   tensors it touches, so the host folds the step into one row of 8 floats (scoef, computed in float64):
+     m_t     = r[0] * x + r[1] * eps                                  (x0 prediction)
+     x_next  = r[2] * x + r[3] * m_t + r[4] * m1 + r[5] * noise       (m1: the previous step's x0 prediction)
+     m1 <- m_t, latents <- x_next
+     next_in = bf16(r[6] * x_next) into channels 0..3 of every copy   (the next step's scale_model_input)
+   r[7] is the input scale of the row's own step (unused by the kernel). guidance scale = coef[row][5] of the shared
+   8-float table. latents, m1 and noise (optional, NULL = none) are fp32 NHWC [batch, hw, 4], 16-byte aligned. */
+typedef struct pp_solver_desc {
+    const void* eps;     /* as pp_unipc_desc: [n_copies*batch, hw, eps_ld] fp32 or bf16, unconditional half first */
+    int32_t eps_fp32;
+    int32_t eps_ld;
+    float* latents;
+    float* m1;
+    const float* noise;
+    const float* coef;   /* [n_steps, 8], column 5 = guidance scale */
+    const float* scoef;  /* [n_steps, 8] */
+    int32_t* step_idx;
+    int32_t advance_step;
+    int32_t do_cfg;
+    int32_t batch, hw;
+    void* next_in;       /* bf16 NHWC [n_copies*batch, hw, next_c]: channels 0..3 refreshed */
+    int32_t next_c, n_copies;
+} pp_solver_desc;
+pp_status pp_solver_step(const pp_solver_desc* d, pp_stream stream);
+
 /* ------------------------------------------------------------------ programs */
 /* A program records op descriptors once (tensor maps are encoded at record time) and
    replays them with one call per denoising step; it can be instantiated as a CUDA graph. */
@@ -413,6 +442,7 @@ pp_status pp_program_add_time_embed(pp_program* p, const float* timesteps,
                                     const int32_t* step_idx, void* out, int32_t batch, int32_t dim);
 pp_status pp_program_add_cfg_ddim(pp_program* p, const pp_cfg_ddim_desc* d);
 pp_status pp_program_add_unipc(pp_program* p, const pp_unipc_desc* d);
+pp_status pp_program_add_solver_step(pp_program* p, const pp_solver_desc* d);
 pp_status pp_program_add_memset(pp_program* p, void* ptr, int64_t bytes);
 pp_status pp_program_add_embed_gather(pp_program* p, const int32_t* idx, const float* base, const float* ext,
                                       const float* pos, void* out, int32_t rows, int32_t vocab, int32_t seq, int32_t dim);

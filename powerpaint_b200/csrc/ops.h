@@ -134,5 +134,7 @@ int cfg_ddim_validate(const pp_cfg_ddim_desc& d);
 int cfg_ddim_launch(const pp_cfg_ddim_desc& d, cudaStream_t s);
 int unipc_validate(const pp_unipc_desc& d);
 int unipc_launch(const pp_unipc_desc& d, cudaStream_t s);
+int solver_validate(const pp_solver_desc& d);
+int solver_launch(const pp_solver_desc& d, cudaStream_t s);
 
 }  // namespace pp

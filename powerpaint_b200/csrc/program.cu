@@ -17,7 +17,7 @@ namespace pp {
 
 enum OpKind {
     OP_GEMM, OP_ATTN, OP_GN, OP_LN, OP_UPSAMPLE, OP_ADD, OP_TIME_EMBED, OP_CFG_DDIM, OP_MEMSET, OP_SOFTMAX, OP_UNIPC, OP_EMBED, OP_CAUSAL_ATTN,
-    OP_WINDOW_COPY, OP_TILE_BLEND
+    OP_WINDOW_COPY, OP_TILE_BLEND, OP_SOLVER
 };
 
 struct LnArgs { const void* x; void* y; const float* gamma; const float* beta; int rows, c; float eps; };
@@ -48,6 +48,7 @@ struct Op {
         pp_unipc_desc unipc;
         WcArgs wc;
         pp_tile_blend_desc tb;
+        pp_solver_desc solver;
     };
     Op() { memset(this, 0, sizeof(*this)); }
 };
@@ -82,6 +83,7 @@ static int run_op(const Op& op, cudaStream_t s) {
         case OP_WINDOW_COPY: return window_copy_launch(op.wc.src, op.wc.dst, op.wc.elem_bytes, op.wc.channels, op.wc.src_pix,
                                                        op.wc.dst_pix, op.wc.windows, op.wc.count, op.wc.max_pixels, s);
         case OP_TILE_BLEND: return tile_blend_launch(op.tb, s);
+        case OP_SOLVER: return solver_launch(op.solver, s);
     }
     set_last_error("program: unknown op kind %d", (int)op.kind);
     return PP_ERR_INVALID;
@@ -92,6 +94,7 @@ static int launches_of(const Op& op) {
         case OP_GN: return 2;  // stats + apply (the stats memset is a memset node, not a kernel)
         case OP_CFG_DDIM: return op.ddim.advance_step ? 2 : 1;
         case OP_UNIPC: return op.unipc.advance_step ? 2 : 1;
+        case OP_SOLVER: return op.solver.advance_step ? 2 : 1;
         case OP_MEMSET: return 0;
         default: return 1;
     }
@@ -234,6 +237,18 @@ pp_status pp_program_add_unipc(pp_program* p, const pp_unipc_desc* d) {
     pp::Op op;
     op.kind = pp::OP_UNIPC;
     op.unipc = *d;
+    p->ops.push_back(op);
+    return pp::PP_OK;
+}
+
+pp_status pp_program_add_solver_step(pp_program* p, const pp_solver_desc* d) {
+    PP_PROG_CHECK(p);
+    if (!d) { pp::set_last_error("pp_program_add_solver_step: null descriptor"); return pp::PP_ERR_INVALID; }
+    int rc = pp::solver_validate(*d);
+    if (rc) return rc;
+    pp::Op op;
+    op.kind = pp::OP_SOLVER;
+    op.solver = *d;
     p->ops.push_back(op);
     return pp::PP_OK;
 }

@@ -118,6 +118,14 @@ class FusedDenoiser:
                                     last_sample=st["last_sample"], m1=st["m1"], m2=st["m2"], coef=coef,
                                     ucoef=st["ucoef"], step_idx=step_idx, advance_step=True, do_cfg=do_cfg, batch=B,
                                     hw=h * w, next_in=x_in, next_c=X_IN_C, n_copies=2 if do_cfg else 1))
+        elif sched == "solver":
+            # DPM-Solver++ / Euler / Euler-ancestral: the previous x0 prediction lives next to the latents
+            st["m1"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
+            st["scoef"] = torch.zeros(MAX_STEPS, 8, dtype=torch.float32, device=dev)
+            prog.add(ops.solver_desc(eps=uplan.outputs["eps"], eps_fp32=True, eps_ld=4, latents=st["latents"],
+                                     m1=st["m1"], coef=coef, scoef=st["scoef"], step_idx=step_idx, advance_step=True,
+                                     do_cfg=do_cfg, batch=B, hw=h * w, noise=st["noise"] if with_noise else None,
+                                     next_in=x_in, next_c=X_IN_C, n_copies=2 if do_cfg else 1))
         else:
             if blend:  # 4-channel UNet: known region kept on the noised original after every step
                 st["blend_x0"] = torch.zeros(h * w, 4, dtype=torch.float32, device=dev)
@@ -139,9 +147,9 @@ class FusedDenoiser:
         return max((s["program"].num_launches for s in self._cache.values()), default=0)
 
     # ------------------------------------------------------------------ run
-    def _fill_x_in(self, st: dict, latents_only: bool = False):
+    def _fill_x_in(self, st: dict, latents_only: bool = False, scale: float = 1.0):
         B, do_cfg, x_in = st["B"], st["do_cfg"], st["x_in"]
-        lat16 = st["latents"].to(torch.bfloat16)
+        lat16 = (st["latents"] * scale if scale != 1.0 else st["latents"]).to(torch.bfloat16)
         for cpy in range(2 if do_cfg else 1):
             x_in[cpy * B:(cpy + 1) * B, :, :4] = lat16
             if not latents_only:
@@ -154,7 +162,7 @@ class FusedDenoiser:
             side_prompt_embeds: Optional[torch.Tensor] = None, control_image: Optional[torch.Tensor] = None,
             side_scale: float = 1.0, side_keep: Optional[Sequence[float]] = None,
             noise_fn: Optional[Callable[[int], torch.Tensor]] = None, ucoef: Optional[torch.Tensor] = None,
-            blend: Optional[dict] = None,
+            scoef: Optional[torch.Tensor] = None, blend: Optional[dict] = None,
             callback: Optional[Callable[[int, int, torch.Tensor], Optional[torch.Tensor]]] = None,
             use_graph: bool = True) -> torch.Tensor:
         """latents [B,4,h,w]; prompt_embeds [nb,77,768] for the UNet (negative half first when CFG);
@@ -163,7 +171,9 @@ class FusedDenoiser:
         for the side net; `side_scale` x `side_keep[i]` (default 1) scales the side net's residuals at step i;
         coef [n,8] from `DDIMScheduler.step_coefficients`; `noise_fn(i)` supplies
         the eta > 0 variance noise of step i; `ucoef` [n,12] (`UniPCMultistepScheduler.unipc_coefficients`) selects
-        the UniPC step kernel instead of DDIM; `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
+        the UniPC step kernel instead of DDIM; `scoef` [n,8] (`solver_coefficients` of DPMSolverMultistepScheduler,
+        EulerDiscreteScheduler, EulerAncestralDiscreteScheduler) selects `pp_solver_step`, with `noise_fn(i)` the
+        noise of a stochastic step and column 7 of row 0 the input scale of the first step; `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
         sqrt_alpha [n]) is the 4-channel-UNet blend (ref pipeline_PowerPaint.py:1025-1035).
         `callback(i, t, latents_nchw)` may return replacement
         latents. Returns the final latents [B,4,h,w] fp32."""
@@ -186,9 +196,13 @@ class FusedDenoiser:
         cur = torch.cuda.current_stream(dev)
         self._stream.wait_stream(cur)
         with torch.cuda.device(dev), torch.cuda.stream(self._stream):
-            sched = "unipc" if ucoef is not None else "ddim"
+            if ucoef is not None and scoef is not None:
+                raise ValueError("ucoef and scoef select different step kernels: pass one")
+            sched = "unipc" if ucoef is not None else "solver" if scoef is not None else "ddim"
             if sched == "unipc" and (noise_fn is not None or blend is not None):
                 raise NotImplementedError("eta / the 4-channel blend are DDIM-only on the fused path")
+            if sched == "solver" and blend is not None:
+                raise NotImplementedError("the 4-channel blend is DDIM-only on the fused path")
             st = self._get(B, h, w, do_cfg, prompt_embeds.shape[1], noise_fn is not None, extra_per_copy, sched,
                            blend is not None)
             if sched == "unipc":
@@ -197,13 +211,21 @@ class FusedDenoiser:
                 st["ucoef"][:n_steps].copy_(ucoef.to(dev, torch.float32))
                 for k in ("last_sample", "m1", "m2"):
                     st[k].zero_()
+            in_scale = lambda i: 1.0  # noqa: E731  (scale_model_input of step i)
+            if sched == "solver":
+                if len(scoef) != n_steps:
+                    raise ValueError("scoef needs one row per step")
+                sc = scoef.to(torch.float32).cpu()
+                st["scoef"][:n_steps].copy_(sc.to(dev))
+                st["m1"].zero_()
+                in_scale = lambda i: float(sc[i, 7]) if i < n_steps else 1.0  # noqa: E731
             # ---- per-call inputs (all outside the loop)
             st["latents"].copy_(ops.nhwc_fp32_from_nchw(latents.to(dev)))
             if extra is not None:
                 st["extra"].copy_(ops.nhwc_fp32_from_nchw(extra.to(dev)))
             else:
                 st["extra"].zero_()
-            self._fill_x_in(st)
+            self._fill_x_in(st, scale=in_scale(0))
             ts = torch.as_tensor([float(t) for t in timesteps], dtype=torch.float32)
             st["timesteps"][:n_steps].copy_(ts.to(dev))
             cf = coef.clone().float()
@@ -247,7 +269,7 @@ class FusedDenoiser:
                         new = callback(i, timesteps[i], cur_lat)
                         if new is not None and new is not cur_lat:
                             st["latents"].copy_(ops.nhwc_fp32_from_nchw(new.to(dev)))
-                            self._fill_x_in(st, latents_only=True)
+                            self._fill_x_in(st, latents_only=True, scale=in_scale(i + 1))
             out = ops.nchw_from_nhwc_fp32(st["latents"], h, w).clone()
         cur.wait_stream(self._stream)
         out.record_stream(cur)

@@ -282,6 +282,19 @@ def unipc_desc(*, eps, eps_fp32, eps_ld, latents, last_sample, m1, m2, coef, uco
     return Desc("unipc", d, (eps, latents, last_sample, m1, m2, coef, ucoef, step_idx, next_in))
 
 
+def solver_desc(*, eps, eps_fp32, eps_ld, latents, m1, coef, scoef, step_idx, advance_step, do_cfg, batch, hw,
+                noise=None, next_in=None, next_c=0, n_copies=0) -> Desc:
+    """pp_solver_step (include/powerpaint_b200.h): CFG + one folded DPM-Solver++ / Euler / Euler-ancestral step"""
+    d = N.SolverDesc()
+    d.eps, d.eps_fp32, d.eps_ld = N.ptr(eps), 1 if eps_fp32 else 0, eps_ld
+    d.latents, d.m1, d.noise = N.ptr(latents), N.ptr(m1), N.ptr(noise)
+    d.coef, d.scoef, d.step_idx = N.ptr(coef), N.ptr(scoef), N.ptr(step_idx)
+    d.advance_step, d.do_cfg = 1 if advance_step else 0, 1 if do_cfg else 0
+    d.batch, d.hw = batch, hw
+    d.next_in, d.next_c, d.n_copies = N.ptr(next_in), next_c, n_copies
+    return Desc("solver", d, (eps, latents, m1, noise, coef, scoef, step_idx, next_in))
+
+
 def _tile_view(t: torch.Tensor, name: str):
     """fp32 [batch, h, w, channels] with every sample contiguous (samples may sit any stride apart)"""
     if t.dtype != torch.float32 or t.dim() != 4 or not t.is_cuda:
@@ -363,6 +376,8 @@ def run(desc: Desc) -> None:
         N.check(L.pp_cfg_ddim_step(C.byref(desc.c), s), "pp_cfg_ddim_step")
     elif desc.kind == "unipc":
         N.check(L.pp_unipc_step(C.byref(desc.c), s), "pp_unipc_step")
+    elif desc.kind == "solver":
+        N.check(L.pp_solver_step(C.byref(desc.c), s), "pp_solver_step")
     elif desc.kind == "tile_blend":
         N.check(L.pp_tile_blend(C.byref(desc.c), s), "pp_tile_blend")
     else:
@@ -493,7 +508,8 @@ class Program:
         L = N.lib()
         fn = {"gemm": L.pp_program_add_gemm, "attn": L.pp_program_add_attention,
               "gn": L.pp_program_add_group_norm, "cfg_ddim": L.pp_program_add_cfg_ddim,
-              "unipc": L.pp_program_add_unipc, "tile_blend": L.pp_program_add_tile_blend}[desc.kind]
+              "unipc": L.pp_program_add_unipc, "tile_blend": L.pp_program_add_tile_blend,
+              "solver": L.pp_program_add_solver_step}[desc.kind]
         N.check(fn(self._h, C.byref(desc.c)), f"pp_program_add_{desc.kind}")
         self._keep.append(desc.keep)
         self.labels.append(desc.kind)

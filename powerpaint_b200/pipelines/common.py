@@ -42,6 +42,24 @@ def randn_tensor(shape, generator=None, device=None, dtype=None):
     return torch.randn(shape, generator=generator, device=rand_device, dtype=dtype).to(device)
 
 
+def solver_loop_inputs(scheduler, timesteps, shape, generator, device):
+    """(scoef, noise_fn, finish) for a scheduler stepped by `pp_solver_step` (kind "solver") over `timesteps`, a
+    suffix of `scheduler.timesteps` (strength < 1). diffusers' `step` draws `randn_tensor(model_output.shape)` once
+    per call: the stochastic variants consume that noise through `noise_fn(i)` (in step order), while Euler's
+    discarded draws are made by `finish()` after the loop, so the generator ends where the reference leaves it."""
+    scoef = scheduler.solver_coefficients(first=len(scheduler.timesteps) - len(timesteps))
+
+    def draw(i):
+        return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+
+    def finish():
+        if scheduler.draws_noise and not scheduler.stochastic:
+            for i in range(len(timesteps)):
+                draw(i)
+
+    return scoef, (draw if scheduler.stochastic else None), finish
+
+
 def prepare_mask_and_masked_image(image, mask, height, width, return_image: bool = False):
     """(mask [B,1,H,W] in {0,1}, masked_image [B,3,H,W] in [-1,1]) from PIL / numpy / tensor inputs;
     same accepted types, range checks and exceptions as the reference (:39-153)."""

@@ -20,7 +20,7 @@ import torch
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import UNet2DConditionModel
 from .common import (StableDiffusionPipelineOutput, decode_latents, encode_text, prepare_mask_and_masked_image,
-                     randn_tensor, uint8_device_inputs, vae_encode)
+                     randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
 
 
 class StableDiffusionInpaintPipeline:
@@ -101,7 +101,8 @@ class StableDiffusionInpaintPipeline:
         """one subfolder of a pipeline directory; `entry` = [library, class name] of model_index.json"""
         from ..loading import load_json
         from ..models import AutoencoderKL, BrushNetModel, ControlNetModel
-        from ..schedulers import DDIMScheduler, UniPCMultistepScheduler
+        from .. import schedulers
+        from ..schedulers import DDIMScheduler
 
         if name == "unet":
             return UNet2DConditionModel.from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
@@ -123,13 +124,14 @@ class StableDiffusionInpaintPipeline:
         if name == "scheduler":
             cfg = load_json(directory, "scheduler_config.json")
             stored = cfg.get("_class_name")
-            if stored == "UniPCMultistepScheduler":
-                return UniPCMultistepScheduler.from_config(cfg)
+            if stored in ("UniPCMultistepScheduler", "DPMSolverMultistepScheduler", "EulerDiscreteScheduler",
+                          "EulerAncestralDiscreteScheduler"):
+                return getattr(schedulers, stored).from_config(cfg)
             if stored not in (None, "DDIMScheduler"):
                 import warnings
 
                 warnings.warn(f"powerpaint_b200: the stored scheduler {stored} is replaced by DDIMScheduler built from "
-                              "the same noise schedule (the fused step kernels implement DDIM and UniPC)", stacklevel=3)
+                              "the same noise schedule (the fused step kernels implement DDIM, UniPC, DPM-Solver++ and Euler)", stacklevel=3)
             return DDIMScheduler.from_config(cfg)
         raise ValueError(f"unknown pipeline component {name!r} ({entry})")
 
@@ -429,8 +431,10 @@ class StableDiffusionInpaintPipeline:
         if not hasattr(self.scheduler, "step_coefficients"):
             raise TypeError("the fused loop needs powerpaint_b200.schedulers.DDIMScheduler (step_coefficients)")
         coef = self.scheduler.step_coefficients(timesteps, eta=extra_step_kwargs.get("eta", 0.0))
-        ucoef = None
-        if getattr(self.scheduler, "kind", "ddim") == "unipc":
+        ucoef = scoef = None
+        finish = None
+        kind = getattr(self.scheduler, "kind", "ddim")
+        if kind == "unipc":
             ucoef = self.scheduler.unipc_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
         blend = None
         if num_channels_unet == 4:
@@ -446,16 +450,23 @@ class StableDiffusionInpaintPipeline:
 
             def noise_fn(i):
                 return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+        if kind == "solver":
+            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
             def cb(i, t, lat):
                 if i % callback_steps == 0:
                     callback(i, t, lat)
                 return None
+        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
+        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, timesteps=timesteps, coef=coef,
                                       guidance_scale=guidance_scale,
                                       extra=torch.cat([mask, masked_image_latents], dim=1) if num_channels_unet == 9
-                                      else None, noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb)
+                                      else None, noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb,
+                                      **({} if scoef is None else dict(scoef=scoef)))
+        if finish is not None:
+            finish()
         image = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
         if not return_dict:
             return (image, None)

@@ -21,7 +21,7 @@ import torch
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import BrushNetModel, UNet2DConditionModel
 from .common import (StableDiffusionPipelineOutput, check_control_guidance, check_image, check_prompt_arguments,
-                     decode_latents, encode_text, preprocess_image, randn_tensor)
+                     decode_latents, encode_text, preprocess_image, randn_tensor, solver_loop_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
 
@@ -286,11 +286,15 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         # device coefficient table the recorded program indexes
         coef = self.scheduler.step_coefficients(ts, eta=extra_step_kwargs.get("eta", 0.0))
         # the v2 app runs UniPC (app.py:197): its folded per-step scalars select the UniPC step kernel
-        ucoef = self.scheduler.unipc_coefficients() if getattr(self.scheduler, "kind", "ddim") == "unipc" else None
+        kind = getattr(self.scheduler, "kind", "ddim")
+        ucoef = self.scheduler.unipc_coefficients() if kind == "unipc" else None
+        scoef = finish = None
         noise_fn = None
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
             def noise_fn(i):
                 return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+        if kind == "solver":
+            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, ts, shape, generator, device)
         cb = None
         if callback_on_step_end is not None or callback is not None:
             pipe = self
@@ -313,11 +317,16 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
                 if callback is not None and i % (callback_steps or 1) == 0:
                     callback(i, t, lat)
                 return new
+        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
+        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds,
                                       timesteps=ts, coef=coef, guidance_scale=guidance_scale,
                                       extra=conditioning_latents, side_scale=float(brushnet_conditioning_scale),
                                       side_keep=keep, ucoef=ucoef,
-                                      noise_fn=noise_fn, callback=cb)
+                                      noise_fn=noise_fn, callback=cb,
+                                      **({} if scoef is None else dict(scoef=scoef)))
+        if finish is not None:
+            finish()
         image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
         if not return_dict:
             return (image_o, None)

@@ -18,7 +18,7 @@ from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import ControlNetModel, UNet2DConditionModel
 from .common import (StableDiffusionPipelineOutput, check_control_guidance, check_image, check_prompt_arguments,
                      decode_latents, prepare_mask_and_masked_image, preprocess_image, randn_tensor,
-                     uint8_device_inputs)
+                     solver_loop_inputs, uint8_device_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
 
@@ -159,8 +159,10 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         # `controlnet_keep` (ref:pipeline_PowerPaint_ControlNet.py:1652-1658): the per-step scale
         # conditioning_scale * keep[i] sits in the device coefficient table the recorded program indexes
         coef = self.scheduler.step_coefficients(timesteps, eta=extra_step_kwargs.get("eta", 0.0))
-        ucoef = None
-        if getattr(self.scheduler, "kind", "ddim") == "unipc":
+        ucoef = scoef = None
+        finish = None
+        kind = getattr(self.scheduler, "kind", "ddim")
+        if kind == "unipc":
             ucoef = self.scheduler.unipc_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
         noise_fn = None
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
@@ -168,18 +170,25 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
 
             def noise_fn(i):
                 return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+        if kind == "solver":
+            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
             def cb(i, t, lat):
                 if i % callback_steps == 0:
                     callback(i, t, lat)
                 return None
+        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
+        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds,
                                       control_image=control, timesteps=timesteps, coef=coef,
                                       guidance_scale=guidance_scale,
                                       extra=torch.cat([mask, masked_image_latents], dim=1),
                                       side_scale=float(controlnet_conditioning_scale), side_keep=keep,
-                                      noise_fn=noise_fn, ucoef=ucoef, callback=cb)
+                                      noise_fn=noise_fn, ucoef=ucoef, callback=cb,
+                                      **({} if scoef is None else dict(scoef=scoef)))
+        if finish is not None:
+            finish()
         image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
         if not return_dict:
             return (image_o, None)
