@@ -29,6 +29,8 @@
  *   pp_unipc_step     CFG combine + UniPCMultistepScheduler.step (the v2 app's scheduler, app.py:197)
  *   pp_solver_step    CFG combine + DPMSolverMultistepScheduler / EulerDiscreteScheduler /
  *                     EulerAncestralDiscreteScheduler.step (the scheduler a user swaps in, as app.py:197 does)
+ *   pp_pool_broadcast spatial mean of a side-net residual, broadcast to full size (global_pool_conditions,
+ *                     BrushNet_CA.py:936-943), added onto an optional running Multi-ControlNet sum
  *   pp_upsample_nearest  Upsample2D with an explicit output size (unet_2d_condition.py:1120-1126,1311-1312)
  *                     Also carries: LayerNorm of BasicTransformerBlock folded into the producing / consuming
  *                     GEMMs (row_stats / ln_stats; diffusers LayerNorm norm1/2/3, SURVEY.md App. A.3), and
@@ -422,6 +424,21 @@ typedef struct pp_solver_desc {
 } pp_solver_desc;
 pp_status pp_solver_step(const pp_solver_desc* d, pp_stream stream);
 
+/* ------------------------------------------------------------------ side-net global pooling */
+/* Global pooling of a side net's residual (`global_pool_conditions`: BrushNet_CA.py:936-943, diffusers
+   ControlNetModel): for every sample s, pixel p and channel c of the bf16 NHWC [batch, hw, channels] buffers
+     out[s, p, c] = bf16(prev[s, p, c] + mean_p x[s, p, c])          (prev == NULL: bf16(mean_p x[s, p, c]))
+   The sum over p is fp32 in a fixed order, so the result is bit-identical from run to run. out is written at full
+   size, so the UNet's consumers of the residual are unchanged; prev adds the residuals of earlier nets of a
+   Multi-ControlNet. channels % 8 == 0; out must not alias x, prev may equal out. */
+typedef struct pp_pool_broadcast_desc {
+    const void* x;
+    const void* prev; /* may be NULL */
+    void* out;
+    int32_t batch, hw, channels;
+} pp_pool_broadcast_desc;
+pp_status pp_pool_broadcast(const pp_pool_broadcast_desc* d, pp_stream stream);
+
 /* ------------------------------------------------------------------ programs */
 /* A program records op descriptors once (tensor maps are encoded at record time) and
    replays them with one call per denoising step; it can be instantiated as a CUDA graph. */
@@ -454,6 +471,7 @@ pp_status pp_program_add_window_copy(pp_program* p, const void* src, void* dst, 
                                      int64_t src_pix, int64_t dst_pix, const pp_window* windows, int32_t count,
                                      int32_t max_pixels);
 pp_status pp_program_add_tile_blend(pp_program* p, const pp_tile_blend_desc* d);
+pp_status pp_program_add_pool_broadcast(pp_program* p, const pp_pool_broadcast_desc* d);
 int32_t pp_program_num_ops(const pp_program* p);
 /* number of kernel launches one run enqueues */
 int32_t pp_program_num_launches(const pp_program* p);

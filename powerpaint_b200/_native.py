@@ -127,6 +127,10 @@ class TileBlendDesc(C.Structure):
     ]
 
 
+class PoolBroadcastDesc(C.Structure):
+    _fields_ = [("x", vp), ("prev", vp), ("out", vp), ("batch", i32), ("hw", i32), ("channels", i32)]
+
+
 # every exported symbol of include/powerpaint_b200.h with (restype, argtypes)
 _SIGNATURES = {
     "pp_last_error": (C.c_char_p, []),
@@ -165,6 +169,8 @@ _SIGNATURES = {
     "pp_program_add_window_copy": (C.c_int, [vp, vp, vp, i32, i32, i64, i64, vp, i32, i32]),
     "pp_tile_blend": (C.c_int, [C.POINTER(TileBlendDesc), vp]),
     "pp_program_add_tile_blend": (C.c_int, [vp, C.POINTER(TileBlendDesc)]),
+    "pp_pool_broadcast": (C.c_int, [C.POINTER(PoolBroadcastDesc), vp]),
+    "pp_program_add_pool_broadcast": (C.c_int, [vp, C.POINTER(PoolBroadcastDesc)]),
     "pp_program_create": (C.c_int, [C.POINTER(vp)]),
     "pp_program_run_range": (C.c_int, [vp, i32, i32, vp]),
     "pp_program_destroy": (None, [vp]),

@@ -17,7 +17,7 @@ namespace pp {
 
 enum OpKind {
     OP_GEMM, OP_ATTN, OP_GN, OP_LN, OP_UPSAMPLE, OP_ADD, OP_TIME_EMBED, OP_CFG_DDIM, OP_MEMSET, OP_SOFTMAX, OP_UNIPC, OP_EMBED, OP_CAUSAL_ATTN,
-    OP_WINDOW_COPY, OP_TILE_BLEND, OP_SOLVER
+    OP_WINDOW_COPY, OP_TILE_BLEND, OP_SOLVER, OP_POOL_BROADCAST
 };
 
 struct LnArgs { const void* x; void* y; const float* gamma; const float* beta; int rows, c; float eps; };
@@ -49,6 +49,7 @@ struct Op {
         WcArgs wc;
         pp_tile_blend_desc tb;
         pp_solver_desc solver;
+        pp_pool_broadcast_desc pool;
     };
     Op() { memset(this, 0, sizeof(*this)); }
 };
@@ -84,6 +85,7 @@ static int run_op(const Op& op, cudaStream_t s) {
                                                        op.wc.dst_pix, op.wc.windows, op.wc.count, op.wc.max_pixels, s);
         case OP_TILE_BLEND: return tile_blend_launch(op.tb, s);
         case OP_SOLVER: return solver_launch(op.solver, s);
+        case OP_POOL_BROADCAST: return pool_broadcast_launch(op.pool, s);
     }
     set_last_error("program: unknown op kind %d", (int)op.kind);
     return PP_ERR_INVALID;
@@ -322,6 +324,18 @@ pp_status pp_program_add_tile_blend(pp_program* p, const pp_tile_blend_desc* d) 
     pp::Op op;
     op.kind = pp::OP_TILE_BLEND;
     op.tb = *d;
+    p->ops.push_back(op);
+    return pp::PP_OK;
+}
+
+pp_status pp_program_add_pool_broadcast(pp_program* p, const pp_pool_broadcast_desc* d) {
+    PP_PROG_CHECK(p);
+    if (!d) { pp::set_last_error("pp_program_add_pool_broadcast: null descriptor"); return pp::PP_ERR_INVALID; }
+    int rc = pp::pool_broadcast_validate(*d);
+    if (rc) return rc;
+    pp::Op op;
+    op.kind = pp::OP_POOL_BROADCAST;
+    op.pool = *d;
     p->ops.push_back(op);
     return pp::PP_OK;
 }

@@ -23,35 +23,54 @@ for it (weights are zero-padded at pack time), so no per-net concat exists. The 
 written once per call; the step kernel only refreshes the four latent channels.
 
 Per-step coefficient row (8 floats, `coef[step]`): 0-4 DDIM (sqrt(a_t), sqrt(1-a_t), sqrt(a_prev),
-sqrt(1-a_prev-sigma^2), sigma), 5 guidance scale, 6 side-net conditioning scale x keep flag of the step
-(`brushnet_keep` / `controlnet_keep`, Brushnet_CA.py:1369-1376,1403-1409, ControlNet.py:1652-1658), 7 spare.
-A recorded plan therefore serves every guidance / conditioning scale and every control_guidance window.
+sqrt(1-a_prev-sigma^2), sigma), 5 guidance scale, 6 spare, 7 the 4-channel blend's sqrt(alpha_bar). The side nets'
+conditioning scale x keep flag of the step (`brushnet_keep` / `controlnet_keep`, Brushnet_CA.py:1369-1376,1403-1409,
+ControlNet.py:1652-1658) sits in a [MAX_STEPS, K] table, one column per side net. A recorded plan therefore serves
+every guidance / conditioning scale and every control_guidance window.
+
+Side-net options (the reference's `guess_mode`, `global_pool_conditions` and MultiControlNetModel):
+- guess mode under CFG: the side net runs on the conditional half only (x_in[B:2B], the conditional prompt rows, B
+  control images) and its zero-convs write the conditional rows of the 2B-row residual buffers the UNet reads. The
+  unconditional rows are zeroed when the plan is recorded and never written again (ControlNet.py:1669-1701,
+  Brushnet_CA.py:1394-1427). Residual k is scaled by the recorded constant logspace(-1, 0, n)[k] (`guess_mode_alphas`).
+- global pooling: a pooled net's residuals are replaced by their spatial mean, broadcast to full size
+  (pp_pool_broadcast); the logspace factors do not apply to it.
+- K ControlNets record into the same program and activation pool, in net order; net k's zero-convs add net k-1's
+  residuals through the epilogue's second residual, so the last net writes the sum the UNet reads.
 """
 from __future__ import annotations
 
 from collections import OrderedDict
-from typing import Callable, Optional, Sequence
+from typing import Callable, Optional
 
 import torch
 
 from . import ops
-from .engine import NetEngine, Plan
+from .engine import NetEngine, Plan, guess_mode_alphas
 
 MAX_STEPS = 1000
 X_IN_C = 16
-COEF_GUIDANCE, COEF_SIDE_SCALE = 5, 6
+COEF_GUIDANCE = 5
 
 
 class FusedDenoiser:
-    """mode: 'v1' (UNet, 9-ch), 'brushnet' (BrushNet + 4-ch UNet), 'controlnet' (ControlNet + 9-ch UNet)"""
+    """mode: 'v1' (UNet, 9-ch), 'brushnet' (BrushNet + 4-ch UNet), 'controlnet' (ControlNet + 9-ch UNet). For
+    'controlnet', `side` may also be a list of ControlNets or a MultiControlNetModel (its `.nets`)."""
 
     def __init__(self, unet, side=None, mode: str = "v1"):
         if mode not in ("v1", "brushnet", "controlnet"):
             raise ValueError(mode)
         if (mode == "v1") != (side is None):
             raise ValueError("side net must be given exactly for modes 'brushnet' / 'controlnet'")
+        sides = list(getattr(side, "nets", side)) if isinstance(side, (list, tuple)) or hasattr(side, "nets") \
+            else ([side] if side is not None else [])
+        if mode == "brushnet" and len(sides) != 1:
+            raise ValueError("mode 'brushnet' takes exactly one BrushNet")
+        if mode == "controlnet" and not sides:
+            raise ValueError("mode 'controlnet' needs at least one ControlNet")
         self.unet = unet
-        self.side = side
+        self.sides = sides
+        self.side = sides[0] if sides else None
         self.mode = mode
         # recorded plans, least recently used first; a plan owns its activation pool (a few GB at C2), so only
         # MAX_PLANS shapes are kept
@@ -62,48 +81,81 @@ class FusedDenoiser:
 
     # ------------------------------------------------------------------ plan
     def _get(self, B: int, h: int, w: int, do_cfg: bool, ctx_len: int, with_noise: bool,
-             extra_per_copy: bool, sched: str = "ddim", blend: bool = False) -> dict:
+             extra_per_copy: bool, sched: str = "ddim", blend: bool = False, guess: bool = False) -> dict:
+        K = len(self.sides)
+        pools = tuple(bool(getattr(s.config, "global_pool_conditions", False)) for s in self.sides)
         # the key carries the parameter generation of each model: `load_state_dict` / `.to()` invalidate it,
         # and the cached entry keeps its engines alive, so a recycled id() can never alias a stale program
-        key = (B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, self.unet.generation,
-               self.side.generation if self.side is not None else -1)
+        key = (B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, K, guess, pools,
+               self.unet.generation, tuple(s.generation for s in self.sides))
         st = self._cache.get(key)
         if st is not None:
             self._cache.move_to_end(key)
             return st
-        for k in [k for k in self._cache if k[-2:] != key[-2:]]:  # (unet generation, side generation)
+        for k in [k for k in self._cache if k[-2:] != key[-2:]]:  # (unet generation, side generations)
             del self._cache[k]  # plans recorded against replaced weights
         while len(self._cache) >= self.MAX_PLANS:
             self._cache.popitem(last=False)
         dev = self.unet.device
         nb = 2 * B if do_cfg else B
+        ns = B if guess and do_cfg else nb  # rows the side nets run on: the conditional half in guess mode
         ue: NetEngine = self.unet.engine()
         prog, ctxprog = ops.Program(), ops.Program()
         x_in = torch.zeros(nb, h * w, X_IN_C, dtype=torch.bfloat16, device=dev)
         timesteps = torch.zeros(MAX_STEPS, dtype=torch.float32, device=dev)
         step_idx = torch.zeros(1, dtype=torch.int32, device=dev)
         coef = torch.zeros(MAX_STEPS, 8, dtype=torch.float32, device=dev)
+        side_scale = torch.zeros(MAX_STEPS, max(K, 1), dtype=torch.float32, device=dev)  # scale x keep per step, net
         pool = Plan()  # the nets of one step share one activation pool
-        shared = dict(program=prog, ctx_program=ctxprog, x_in=x_in, timesteps=timesteps, step_idx=step_idx, pool=pool,
-                      scale_dev=(coef[:, COEF_SIDE_SCALE], step_idx, 8))
-        st = dict(B=B, nb=nb, h=h, w=w, do_cfg=do_cfg, x_in=x_in, timesteps=timesteps, step_idx=step_idx, coef=coef,
-                  program=prog, ctx_program=ctxprog, graph=False, with_noise=with_noise,
-                  extra_per_copy=extra_per_copy, engines=(ue, self.side.engine() if self.side is not None else None))
-        side_plan: Optional[Plan] = None
+        shared = dict(program=prog, ctx_program=ctxprog, x_in=x_in, timesteps=timesteps, step_idx=step_idx, pool=pool)
+        st = dict(B=B, nb=nb, ns=ns, h=h, w=w, do_cfg=do_cfg, x_in=x_in, timesteps=timesteps, step_idx=step_idx,
+                  coef=coef, side_scale=side_scale, program=prog, ctx_program=ctxprog, graph=False,
+                  with_noise=with_noise, extra_per_copy=extra_per_copy,
+                  engines=(ue,) + tuple(s.engine() for s in self.sides))
+        side_x = x_in[nb - ns:]  # contiguous: the CFG halves are stacked [uncond; cond]
+        down_s, mid_s, up_s = ue._state_shapes(nb, h, w)
+
+        def residuals(shapes):  # 2B-row buffers the UNet reads; rows the side nets never write stay zero
+            return [torch.zeros(nb, hh * ww, c, dtype=torch.bfloat16, device=dev) for (c, hh, ww) in shapes]
+
+        def rows(bufs):  # the rows the side nets write
+            return [b[nb - ns:].reshape(-1, b.shape[-1]) for b in bufs]
+
+        def side_shared(k):
+            return dict(shared, x_in=side_x, scale_dev=(side_scale[:, k], step_idx, K))
+
+        side_plans = []
+        res_bytes = 0
         if self.mode == "brushnet":
-            se: NetEngine = self.side.engine()
-            side_plan = se._build_plan(nb, h, w, ctx_len, False, False, True, 0, shared=shared)
-            se.append_brushnet_outputs(side_plan, 1.0, scale_dev=shared["scale_dev"])
-            shared_u = dict(shared, adds=(side_plan.outputs["down"], side_plan.outputs["mid"], side_plan.outputs["up"]))
-            uplan = ue._build_plan(nb, h, w, ctx_len, True, False, True, 0, shared=shared_u)
+            se: NetEngine = self.sides[0].engine()
+            side_plan = se._build_plan(ns, h, w, ctx_len, False, False, True, 0, shared=side_shared(0))
+            adds_d, add_m, adds_u = residuals(down_s), residuals([mid_s])[0], residuals(up_s)
+            res_bytes = sum(t.numel() * 2 for t in adds_d + [add_m] + adds_u)
+            alphas = guess_mode_alphas(len(adds_d) + 1 + len(adds_u)) if guess and not pools[0] else None
+            se.append_brushnet_outputs(side_plan, 1.0, targets=(rows(adds_d), rows([add_m])[0], rows(adds_u)),
+                                       scale_dev=(side_scale[:, 0], step_idx, K), alphas=alphas, pool=pools[0])
+            side_plans.append(side_plan)
+            uplan = ue._build_plan(nb, h, w, ctx_len, True, False, True, 0, shared=dict(shared, adds=(adds_d, add_m, adds_u)))
+            st["residuals"] = adds_d + [add_m] + adds_u
         elif self.mode == "controlnet":
-            se = self.side.engine()
-            side_plan = se._build_plan(nb, h, w, ctx_len, False, False, True, 0, shared=shared)
-            shared_u = dict(shared, cn=(side_plan.outputs["down"], side_plan.outputs["mid"]))
-            uplan = ue._build_plan(nb, h, w, ctx_len, False, True, True, 0, shared=shared_u)
+            cn_d, cn_m = residuals(down_s), residuals([mid_s])[0]
+            res_bytes = sum(t.numel() * 2 for t in cn_d + [cn_m])
+            prev = None
+            for k, net in enumerate(self.sides):
+                last = k == K - 1
+                alphas = guess_mode_alphas(len(cn_d) + 1) if guess and not pools[k] else None
+                sp = net.engine()._build_plan(ns, h, w, ctx_len, False, False, True, 0,
+                                              shared=dict(side_shared(k), side_alphas=alphas, side_pool=pools[k],
+                                                          side_targets=(rows(cn_d), rows([cn_m])[0]) if last else None,
+                                                          side_prev=prev))
+                prev = (sp.outputs["down"], sp.outputs["mid"])
+                side_plans.append(sp)
+            uplan = ue._build_plan(nb, h, w, ctx_len, False, True, True, 0, shared=dict(shared, cn=(cn_d, cn_m)))
+            st["residuals"] = cn_d + [cn_m]
         else:
             uplan = ue._build_plan(nb, h, w, ctx_len, False, False, True, 0, shared=shared)
-        st["uplan"], st["side_plan"] = uplan, side_plan
+        st["uplan"], st["side_plans"] = uplan, side_plans
+        st["side_plan"] = side_plans[0] if side_plans else None
         # fp32 master latents and the constant channels (channels-last)
         n_extra = nb if extra_per_copy else B
         st["latents"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
@@ -138,7 +190,7 @@ class FusedDenoiser:
                                        next_c=X_IN_C, n_copies=2 if do_cfg else 1, extra=None, extra_c=0,
                                        blend_x0=st.get("blend_x0"), blend_mask=st.get("blend_mask"),
                                        blend_noise=st.get("blend_noise")))
-        st["bytes"] = uplan.bytes + (side_plan.bytes if side_plan else 0)
+        st["bytes"] = uplan.bytes + sum(p.bytes for p in side_plans) + res_bytes
         self._cache[key] = st
         return st
 
@@ -160,11 +212,11 @@ class FusedDenoiser:
     def run(self, *, latents: torch.Tensor, prompt_embeds: torch.Tensor, timesteps, coef: torch.Tensor,
             guidance_scale: float, extra: Optional[torch.Tensor] = None,
             side_prompt_embeds: Optional[torch.Tensor] = None, control_image: Optional[torch.Tensor] = None,
-            side_scale: float = 1.0, side_keep: Optional[Sequence[float]] = None,
+            side_scale=1.0, side_keep=None,
             noise_fn: Optional[Callable[[int], torch.Tensor]] = None, ucoef: Optional[torch.Tensor] = None,
             scoef: Optional[torch.Tensor] = None, blend: Optional[dict] = None,
             callback: Optional[Callable[[int, int, torch.Tensor], Optional[torch.Tensor]]] = None,
-            use_graph: bool = True) -> torch.Tensor:
+            use_graph: bool = True, guess_mode: bool = False) -> torch.Tensor:
         """latents [B,4,h,w]; prompt_embeds [nb,77,768] for the UNet (negative half first when CFG);
         extra [B or nb,5,h,w] = constant channels (v1/controlnet: mask + masked-image latents;
         brushnet: conditioning latents + mask; nb rows = one set per CFG half); side_prompt_embeds
@@ -176,7 +228,11 @@ class FusedDenoiser:
         noise of a stochastic step and column 7 of row 0 the input scale of the first step; `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
         sqrt_alpha [n]) is the 4-channel-UNet blend (ref pipeline_PowerPaint.py:1025-1035).
         `callback(i, t, latents_nchw)` may return replacement
-        latents. Returns the final latents [B,4,h,w] fp32."""
+        latents. Returns the final latents [B,4,h,w] fp32.
+        K ControlNets: `side_scale` a list of K floats, `side_keep` None or a list of K per-step lists,
+        `control_image` a list of K tensors. `guess_mode`: the side nets' residuals are scaled by logspace(-1, 0, n)
+        (pooled nets excepted) and, under CFG, the side nets see only the conditional half: `side_prompt_embeds` may
+        then be the 2B rows (the conditional B are used) or B rows, control images have B rows."""
         B, _, h, w = latents.shape
         nb = prompt_embeds.shape[0]
         do_cfg = nb == 2 * B
@@ -191,8 +247,15 @@ class FusedDenoiser:
         dev = self.unet.device
         if self._stream is None:
             self._stream = torch.cuda.Stream(device=dev)
-        if side_keep is not None and len(side_keep) != n_steps:
-            raise ValueError("side_keep needs one entry per step")
+        K = len(self.sides)
+        multi = isinstance(side_scale, (list, tuple))
+        scales = [float(v) for v in side_scale] if multi else [float(side_scale)] * max(K, 1)
+        keeps = (list(side_keep) if multi else [side_keep]) if side_keep is not None else [None] * len(scales)
+        if K and (len(scales) != K or len(keeps) != K or (K > 1 and not multi)):
+            raise ValueError(f"{K} side nets: side_scale and side_keep need one entry per net")
+        for kp in keeps:
+            if kp is not None and len(kp) != n_steps:
+                raise ValueError("side_keep needs one entry per step")
         cur = torch.cuda.current_stream(dev)
         self._stream.wait_stream(cur)
         with torch.cuda.device(dev), torch.cuda.stream(self._stream):
@@ -204,7 +267,7 @@ class FusedDenoiser:
             if sched == "solver" and blend is not None:
                 raise NotImplementedError("the 4-channel blend is DDIM-only on the fused path")
             st = self._get(B, h, w, do_cfg, prompt_embeds.shape[1], noise_fn is not None, extra_per_copy, sched,
-                           blend is not None)
+                           blend is not None, bool(guess_mode) and K > 0)
             if sched == "unipc":
                 if len(ucoef) != n_steps:
                     raise ValueError("ucoef needs one row per step")
@@ -230,8 +293,11 @@ class FusedDenoiser:
             st["timesteps"][:n_steps].copy_(ts.to(dev))
             cf = coef.clone().float()
             cf[:, COEF_GUIDANCE] = float(guidance_scale)
-            keep = torch.ones(n_steps) if side_keep is None else torch.tensor([float(k) for k in side_keep])
-            cf[:, COEF_SIDE_SCALE] = float(side_scale) * keep
+            ss = torch.zeros(n_steps, max(K, 1))
+            for k, (scale, kp) in enumerate(zip(scales, keeps)):
+                keep = torch.ones(n_steps) if kp is None else torch.tensor([float(v) for v in kp])
+                ss[:, k] = scale * keep
+            st["side_scale"][:n_steps].copy_(ss.to(dev))
             if blend is not None:
                 cf[:, 7] = torch.as_tensor(blend["sqrt_alpha"], dtype=torch.float32)
                 st["blend_x0"].copy_(ops.nhwc_fp32_from_nchw(blend["x0"][:1].to(dev))[0])
@@ -240,16 +306,20 @@ class FusedDenoiser:
             st["coef"][:n_steps].copy_(cf.to(dev))
             st["step_idx"].zero_()
             st["uplan"].inputs["ctx"].copy_(prompt_embeds.to(dev, torch.bfloat16))
-            if st["side_plan"] is not None:
+            if st["side_plans"]:
                 if side_prompt_embeds is None:
                     raise ValueError("side_prompt_embeds required")
-                st["side_plan"].inputs["ctx"].copy_(side_prompt_embeds.to(dev, torch.bfloat16))
-                if self.mode == "controlnet":
-                    if control_image is None:
-                        raise ValueError("control_image required")
-                    ci = st["side_plan"].inputs["cond_in"]
-                    ci.copy_(ops.nchw_to_nhwc(control_image.to(dev).float().contiguous(), ci.shape[-1]).view_as(ci))
-                    st["side_plan"].cond_program.run()
+                ns = st["ns"]
+                spe = side_prompt_embeds[-ns:] if side_prompt_embeds.shape[0] == nb else side_prompt_embeds
+                images = control_image if isinstance(control_image, (list, tuple)) else [control_image]
+                if self.mode == "controlnet" and (control_image is None or len(images) != K):
+                    raise ValueError(f"control_image required: one per ControlNet ({K})")
+                for k, sp in enumerate(st["side_plans"]):
+                    sp.inputs["ctx"].copy_(spe.to(dev, torch.bfloat16))
+                    if self.mode == "controlnet":
+                        ci = sp.inputs["cond_in"]
+                        ci.copy_(ops.nchw_to_nhwc(images[k].to(dev).float().contiguous(), ci.shape[-1]).view_as(ci))
+                        sp.cond_program.run()
             st["ctx_program"].run()
             # ---- the loop
             prog = st["program"]

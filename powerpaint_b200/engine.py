@@ -63,6 +63,13 @@ class NetConfig:
     conditioning_embedding_out_channels: Tuple[int, ...] = (16, 32, 96, 256)
 
 
+def guess_mode_alphas(n: int) -> Tuple[float, ...]:
+    """The per-residual factors of a side net in guess mode, `torch.logspace(-1, 0, n)` in fp32 (0.1 to 1.0):
+    n = 13 for a ControlNet (12 down + mid), 28 for a BrushNet (12 down + mid + 15 up). BrushNet_CA.py:905-934 and
+    diffusers' ControlNetModel multiply residual k by logspace[k] x conditioning_scale."""
+    return tuple(float(v) for v in torch.logspace(-1, 0, n, dtype=torch.float32))
+
+
 class Plan:
     """A recorded forward for fixed (batch, h, w): programs + the static buffers they touch."""
 
@@ -519,16 +526,22 @@ class NetEngine:
 
     def plan(self, nb: int, h: int, w: int, ctx_len: int = 77, *, with_brushnet_adds: bool = False,
              with_controlnet_res: bool = False, use_step_table: bool = False, n_steps: int = 0,
-             brushnet_outputs: bool = False) -> Plan:
-        key = (nb, h, w, ctx_len, with_brushnet_adds, with_controlnet_res, use_step_table, n_steps, brushnet_outputs)
+             brushnet_outputs: bool = False, side_alphas: Optional[Tuple[float, ...]] = None,
+             side_pool: bool = False) -> Plan:
+        """`side_alphas` / `side_pool`: the side net's per-residual factors and global pooling (`_zero_convs`)"""
+        key = (nb, h, w, ctx_len, with_brushnet_adds, with_controlnet_res, use_step_table, n_steps, brushnet_outputs,
+               side_alphas, side_pool)
         p = self._plans.pop(key, None)
         if p is None:
-            p = self._build_plan(nb, h, w, ctx_len, with_brushnet_adds, with_controlnet_res, use_step_table, n_steps)
+            shared = dict(side_alphas=side_alphas, side_pool=side_pool)
+            p = self._build_plan(nb, h, w, ctx_len, with_brushnet_adds, with_controlnet_res, use_step_table, n_steps,
+                                 shared=shared)
             if self.kind in ("brushnet", "controlnet") and p.scale_dev is None:
                 # eager forward: conditioning_scale is read from a device scalar at run time
                 p.scale_dev = torch.ones(1, dtype=torch.float32, device=self.device)
             if brushnet_outputs:
-                self.append_brushnet_outputs(p, 1.0, scale_dev=(p.scale_dev, None, 0))
+                self.append_brushnet_outputs(p, 1.0, scale_dev=(p.scale_dev, None, 0), alphas=side_alphas,
+                                             pool=side_pool)
             while len(self._plans) >= self.MAX_PLANS:
                 self._plans.pop(next(iter(self._plans)))
         self._plans[key] = p  # most recently used last
@@ -571,7 +584,9 @@ class NetEngine:
         first channels are this net's input; extra channels meet zero weights), `timesteps`,
         `step_idx`, `plan` (record into an existing Plan so that the nets share one buffer pool), and for the
         UNet `adds` = (down, mid, up) / `cn` = (down, mid) buffers produced by the side net;
-        `scale_dev` = (tensor, step_idx, stride): device-side conditioning scale of the side net."""
+        `scale_dev` = (tensor, step_idx, stride): device-side conditioning scale of the side net; for the ControlNet
+        `side_alphas`, `side_pool`, `side_targets` = (down, mid) buffers to write the residuals into and `side_prev` =
+        (down, mid) residuals of the previous net of a Multi-ControlNet to add (`_zero_convs`)."""
         shared = shared or {}
         cfg = self.cfg
         boc = cfg.block_out_channels
@@ -749,18 +764,14 @@ class NetEngine:
             sdev, sstep, sstride = shared.get("scale_dev") or (plan.scale_dev, None, 0)
             if sdev is None:
                 sdev = plan.scale_dev = torch.ones(1, dtype=torch.float32, device=self.device)
-            outs_down = []
-            for k, st in enumerate(states_down):
-                c = st.shape[-1]
-                o = persistent(st.numel() // c, c)
-                outs_down.append(self._linear(plan, prog, st, st.numel() // c, f"controlnet_down_blocks.{k}", c,
-                                              bias=self.vec(f"controlnet_down_blocks.{k}.bias"), out=o,
-                                              alpha_dev=sdev, alpha_step=sstep, alpha_stride=sstride))
-            o = persistent(state_mid.numel() // cm, cm)
-            out_mid = self._linear(plan, prog, state_mid, state_mid.numel() // cm, "controlnet_mid_block",
-                                   cm, bias=self.vec("controlnet_mid_block.bias"), out=o,
-                                   alpha_dev=sdev, alpha_step=sstep, alpha_stride=sstride)
-            plan.outputs["down"], plan.outputs["mid"] = outs_down, out_mid
+            t_down, t_mid = shared.get("side_targets") or ([None] * len(states_down), None)
+            p_down, p_mid = shared.get("side_prev") or ([None] * len(states_down), None)
+            names = [f"controlnet_down_blocks.{k}" for k in range(len(states_down))] + ["controlnet_mid_block"]
+            outs = self._zero_convs(plan, prog, nb, list(zip(states_down + [state_mid], names, list(t_down) + [t_mid],
+                                                             list(p_down) + [p_mid])),
+                                    alphas=shared.get("side_alphas"), pool=shared.get("side_pool", False),
+                                    scale_dev=(sdev, sstep, sstride))
+            plan.outputs["down"], plan.outputs["mid"] = outs[:-1], outs[-1]
             for st in states_down + [state_mid]:
                 self._free(plan, st)
             return plan
@@ -823,30 +834,57 @@ class NetEngine:
         return plan
 
     # ------------------------------------------------------------------ BrushNet zero-convs
-    def append_brushnet_outputs(self, plan: Plan, conditioning_scale: float = 1.0, targets=None, scale_dev=None):
-        """1x1 zero-convs x conditioning_scale on the 12 + 1 + 15 captured states
-        (BrushNet_CA.py:843-845, :861, :900-902, :930-934). `targets` = (down, mid, up) buffer
-        lists of a UNet plan (`with_brushnet_adds=True`) to write straight into. `scale_dev` =
-        (tensor, step_idx, stride): the scale is multiplied by tensor[*step_idx * stride] on the device, so one
-        recorded program serves every `brushnet_conditioning_scale` and the per-step `brushnet_keep` flags
-        (pipeline_PowerPaint_Brushnet_CA.py:1369-1376,1403-1409)."""
-        states_down, state_mid, states_up = plan.outputs["states"]
-        prog = plan.program
+    def _zero_convs(self, plan: Plan, prog, nb: int, items, *, alphas=None, pool: bool = False, scale_dev=None,
+                    conditioning_scale: float = 1.0):
+        """The 1x1 zero-convs of a side net. `items` = [(state, weight name, target, prev)] in residual order;
+        residual k is
+            out_k = a_k * dev * (W_k state_k + b_k) + prev_k,   a_k = conditioning_scale * alphas[k]
+        with dev = scale_dev[0][*scale_dev[1] * scale_dev[2]] read on the device (conditioning scale x keep flag of
+        the step). `alphas`: guess mode's logspace(-1, 0, n) factors (None: 1). `pool`: the scaled zero-conv output
+        is replaced by its spatial mean, broadcast to full size (pp_pool_broadcast), before prev_k is added.
+        `target` None: a fresh buffer that is never recycled; `prev` None: nothing is added. Returns the outputs."""
         sdev, sstep, sstride = scale_dev or (None, None, 0)
-
-        def zc(st, wname, out):
+        outs = []
+        for k, (st, wname, out, prev) in enumerate(items):
             c = st.shape[-1]
             M = st.numel() // c
             if out is None:  # read by the caller / by another net's ops: never recycled
                 out = torch.empty(M, c, dtype=BF16, device=self.device)
                 plan.bytes += out.numel() * 2
-            return self._linear(plan, prog, st, M, wname, c, bias=self.vec(wname + ".bias"), alpha=conditioning_scale,
-                                out=out, alpha_dev=sdev, alpha_step=sstep, alpha_stride=sstride)
-        t_down, t_mid, t_up = targets if targets is not None else (None, None, None)
-        outs_down = [zc(st, f"brushnet_down_blocks.{k}", t_down[k] if t_down else None) for k, st in enumerate(states_down)]
-        out_mid = zc(state_mid, "brushnet_mid_block", t_mid)
-        outs_up = [zc(st, f"brushnet_up_blocks.{k}", t_up[k] if t_up else None) for k, st in enumerate(states_up)]
-        plan.outputs["down"], plan.outputs["mid"], plan.outputs["up"] = outs_down, out_mid, outs_up
+            kw = dict(bias=self.vec(wname + ".bias"), alpha=conditioning_scale * (alphas[k] if alphas else 1.0),
+                      alpha_dev=sdev, alpha_step=sstep, alpha_stride=sstride)
+            if pool:
+                z = self._buf(plan, M, c)
+                self._linear(plan, prog, st, M, wname, c, out=z, **kw)
+                shape = (nb, M // nb, c)
+                prog.add(ops.pool_broadcast_desc(z.view(shape), out.view(shape),
+                                                 None if prev is None else prev.view(shape)))
+                self._free(plan, z)
+            else:
+                self._linear(plan, prog, st, M, wname, c, out=out, res2=prev, **kw)
+            outs.append(out)
+        return outs
+
+    def append_brushnet_outputs(self, plan: Plan, conditioning_scale: float = 1.0, targets=None, scale_dev=None,
+                                alphas=None, pool: bool = False):
+        """1x1 zero-convs x conditioning_scale on the 12 + 1 + 15 captured states
+        (BrushNet_CA.py:843-845, :861, :900-902, :930-934). `targets` = (down, mid, up) buffer
+        lists of a UNet plan (`with_brushnet_adds=True`) to write straight into. `scale_dev` =
+        (tensor, step_idx, stride): the scale is multiplied by tensor[*step_idx * stride] on the device, so one
+        recorded program serves every `brushnet_conditioning_scale` and the per-step `brushnet_keep` flags
+        (pipeline_PowerPaint_Brushnet_CA.py:1369-1376,1403-1409). `alphas` (28 guess-mode factors) and `pool`
+        (`global_pool_conditions`, :936-943): see `_zero_convs`."""
+        states_down, state_mid, states_up = plan.outputs["states"]
+        nd, nu = len(states_down), len(states_up)
+        t_down, t_mid, t_up = targets if targets is not None else ([None] * nd, None, [None] * nu)
+        names = ([f"brushnet_down_blocks.{k}" for k in range(nd)] + ["brushnet_mid_block"]
+                 + [f"brushnet_up_blocks.{k}" for k in range(nu)])
+        nb = states_down[0].shape[0]
+        outs = self._zero_convs(plan, plan.program, nb,
+                                list(zip(states_down + [state_mid] + states_up, names,
+                                         list(t_down) + [t_mid] + list(t_up), [None] * (nd + 1 + nu))),
+                                alphas=alphas, pool=pool, scale_dev=scale_dev, conditioning_scale=conditioning_scale)
+        plan.outputs["down"], plan.outputs["mid"], plan.outputs["up"] = outs[:nd], outs[nd], outs[nd + 1:]
         plan.outputs["conditioning_scale"] = conditioning_scale
         for st in states_down + [state_mid] + states_up:  # every reader of the captured states is recorded
             self._free(plan, st)

@@ -88,6 +88,8 @@ def load_weights(directory: str, variant: Optional[str] = None, stem: str = "dif
 def net_config_from_diffusers(cfg: dict, kind: str) -> NetConfig:
     """diffusers `config.json` -> NetConfig; options the hot path does not implement are refused by name"""
     for k, want in _FIXED.items():
+        if k == "global_pool_conditions" and kind in ("controlnet", "brushnet"):
+            continue  # side nets pool their residuals on the kernel path (pp_pool_broadcast)
         if k in cfg and cfg[k] != want and not (isinstance(want, float) and float(cfg[k]) == want):
             raise NotImplementedError(f"config.{k} = {cfg[k]!r}: the hot path implements {want!r} only (SD-1.5 family)")
     oca = cfg.get("only_cross_attention", False)

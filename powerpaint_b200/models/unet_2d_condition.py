@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops
-from ..engine import NetConfig, NetEngine
+from ..engine import NetConfig, NetEngine, guess_mode_alphas
 from .spec import param_shapes, synthetic_state_dict
 
 
@@ -134,7 +134,10 @@ class _HotPathModel(nn.Module):
         from ..loading import net_config_from_diffusers
 
         d = dict(vars(config)) if not isinstance(config, dict) else dict(config)
-        return cls(net_config_from_diffusers(d, cls.KIND), sample_size=d.get("sample_size") or 64, **kw)
+        m = cls(net_config_from_diffusers(d, cls.KIND), sample_size=d.get("sample_size") or 64, **kw)
+        if cls.KIND != "unet":
+            m.config.global_pool_conditions = bool(d.get("global_pool_conditions", False))
+        return m
 
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, subfolder: Optional[str] = None, torch_dtype=None,
@@ -224,6 +227,26 @@ class _HotPathModel(nn.Module):
         plan.ctx_program.run()
 
     @staticmethod
+    def _nhwc_like(src: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+        """a caller's NCHW residual as the NHWC buffer `dst`; a globally pooled [B, C, 1, 1] residual is broadcast
+        over the pixels, as the reference's `sample + residual` does"""
+        src = src.float()
+        if src.shape[2:] == (1, 1) and dst.shape[1] != 1:
+            return src.reshape(src.shape[0], 1, src.shape[1]).expand(-1, dst.shape[1], -1).to(dst.dtype)
+        return ops.nchw_to_nhwc(src.contiguous()).view_as(dst)
+
+    def _side_plan_options(self, guess_mode: bool, n_res: int):
+        """(per-residual factors, pool) of a side net's forward: the logspace(-1, 0, n_res) factors in guess mode
+        unless the net pools (the reference never applies them to a pooled net)"""
+        pool = bool(self.config.global_pool_conditions)
+        return (guess_mode_alphas(n_res) if guess_mode and not pool else None), pool
+
+    @staticmethod
+    def _pooled(t: torch.Tensor) -> torch.Tensor:
+        """the [B, C, 1, 1] mean the reference returns for a pooled net (every pixel of `t` holds it)"""
+        return t[:, :, :1, :1].contiguous()
+
+    @staticmethod
     def _to_nchw(t: torch.Tensor, nb, h, w, dtype) -> torch.Tensor:
         c = t.shape[-1]
         return ops.nhwc_to_nchw(t.view(nb, h, w, c)).to(dtype)
@@ -280,19 +303,17 @@ class UNet2DConditionModel(_HotPathModel):
             # the reference consumes the lists with pop(0) (unet_2d_condition.py:1223,:1232-1253,:1316-1339)
             for dst in plan.inputs["adds_down"]:
                 src = down_block_add_samples.pop(0)
-                dst.copy_(ops.nchw_to_nhwc(src.float().contiguous()).view_as(dst))
-            plan.inputs["add_mid"].copy_(
-                ops.nchw_to_nhwc(mid_block_add_sample.float().contiguous()).view_as(plan.inputs["add_mid"]))
+                dst.copy_(self._nhwc_like(src, dst))
+            plan.inputs["add_mid"].copy_(self._nhwc_like(mid_block_add_sample, plan.inputs["add_mid"]))
             for dst in plan.inputs["adds_up"]:
                 src = up_block_add_samples.pop(0)
-                dst.copy_(ops.nchw_to_nhwc(src.float().contiguous()).view_as(dst))
+                dst.copy_(self._nhwc_like(src, dst))
         if is_controlnet:
             if len(down_block_additional_residuals) != len(plan.inputs["cn_down"]):
                 raise ValueError("wrong number of down_block_additional_residuals")
             for dst, src in zip(plan.inputs["cn_down"], down_block_additional_residuals):
-                dst.copy_(ops.nchw_to_nhwc(src.float().contiguous()).view_as(dst))
-            plan.inputs["cn_mid"].copy_(
-                ops.nchw_to_nhwc(mid_block_additional_residual.float().contiguous()).view_as(plan.inputs["cn_mid"]))
+                dst.copy_(self._nhwc_like(src, dst))
+            plan.inputs["cn_mid"].copy_(self._nhwc_like(mid_block_additional_residual, plan.inputs["cn_mid"]))
         plan.program.launch()
         out = self._to_nchw(plan.outputs["eps"], nb, h, w, self.dtype)
         if not return_dict:
@@ -347,23 +368,28 @@ class BrushNetModel(_HotPathModel):
                 added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, guess_mode: bool = False,
                 return_dict: bool = True):
-        if guess_mode:
-            raise NotImplementedError("guess_mode is outside the PowerPaint hot path (unused by app.py)")
+        """`guess_mode` and `config.global_pool_conditions` as BrushNet_CA.py:905-943: in guess mode residual k is
+        scaled by logspace(-1, 0, 28)[k] x conditioning_scale; a pooled net skips those factors and returns the
+        spatial mean of each residual, [B, C, 1, 1]."""
         for name, v in (("class_labels", class_labels), ("timestep_cond", timestep_cond),
                         ("attention_mask", attention_mask), ("added_cond_kwargs", added_cond_kwargs)):
             if v is not None:
                 raise NotImplementedError(f"`{name}` is outside the PowerPaint SD-1.5 hot path")
         nb, _, h, w = sample.shape
         with torch.cuda.device(self.device):
+            shapes_d, shape_m, shapes_u = self.engine()._state_shapes(nb, h, w)
+            alphas, pool = self._side_plan_options(guess_mode, len(shapes_d) + 1 + len(shapes_u))
             # one recorded program for every conditioning_scale: the zero-conv epilogues read it from a device scalar
-            plan = self.engine().plan(nb, h, w, encoder_hidden_states.shape[1], brushnet_outputs=True)
+            plan = self.engine().plan(nb, h, w, encoder_hidden_states.shape[1], brushnet_outputs=True,
+                                      side_alphas=alphas, side_pool=pool)
             plan.scale_dev.fill_(float(conditioning_scale))
             self._load_inputs(plan, sample, timestep, encoder_hidden_states, extra_channels=brushnet_cond)
             plan.program.launch()
-            shapes_d, shape_m, shapes_u = self.engine()._state_shapes(nb, h, w)
             down = [self._to_nchw(t, nb, s[1], s[2], self.dtype) for t, s in zip(plan.outputs["down"], shapes_d)]
             mid = self._to_nchw(plan.outputs["mid"], nb, shape_m[1], shape_m[2], self.dtype)
             up = [self._to_nchw(t, nb, s[1], s[2], self.dtype) for t, s in zip(plan.outputs["up"], shapes_u)]
+            if pool:
+                down, mid, up = [self._pooled(t) for t in down], self._pooled(mid), [self._pooled(t) for t in up]
         if not return_dict:
             return (down, mid, up)
         return BrushNetOutput(down_block_res_samples=down, mid_block_res_sample=mid, up_block_res_samples=up)
@@ -386,14 +412,18 @@ class ControlNetModel(_HotPathModel):
                 added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
                 cross_attention_kwargs: Optional[Dict[str, Any]] = None, guess_mode: bool = False,
                 return_dict: bool = True):
-        if guess_mode:
-            raise NotImplementedError("guess_mode is outside the PowerPaint hot path")
+        """`guess_mode` and `config.global_pool_conditions` as diffusers 0.27.0 `ControlNetModel.forward` (restated
+        as recalled, not copied): in guess mode residual k of the 12 down + mid residuals is scaled by
+        logspace(-1, 0, 13)[k] x conditioning_scale; a pooled net skips those factors and returns the spatial mean
+        of each residual, [B, C, 1, 1]."""
         nb, _, h, w = sample.shape
         if tuple(controlnet_cond.shape[2:]) != (8 * h, 8 * w):
             raise ValueError("controlnet_cond must be 8x the latent resolution")
         with torch.cuda.device(self.device):
             eng = self.engine()
-            plan = eng.plan(nb, h, w, encoder_hidden_states.shape[1])
+            shapes_d, shape_m, _ = eng._state_shapes(nb, h, w)
+            alphas, pool = self._side_plan_options(guess_mode, len(shapes_d) + 1)
+            plan = eng.plan(nb, h, w, encoder_hidden_states.shape[1], side_alphas=alphas, side_pool=pool)
             # t-independent (SURVEY.md App. C (3)): the 8-conv embedding is re-run only when the staged control
             # image actually differs (content comparison on the device; an address is not an identity)
             ci = plan.inputs["cond_in"]
@@ -405,9 +435,51 @@ class ControlNetModel(_HotPathModel):
             plan.scale_dev.fill_(float(conditioning_scale))
             self._load_inputs(plan, sample, timestep, encoder_hidden_states)
             plan.program.launch()
-            shapes_d, shape_m, _ = eng._state_shapes(nb, h, w)
             down = [self._to_nchw(t, nb, sh[1], sh[2], self.dtype) for t, sh in zip(plan.outputs["down"], shapes_d)]
             mid = self._to_nchw(plan.outputs["mid"], nb, shape_m[1], shape_m[2], self.dtype)
+            if pool:
+                down, mid = [self._pooled(t) for t in down], self._pooled(mid)
         if not return_dict:
             return (down, mid)
         return ControlNetOutput(down_block_res_samples=down, mid_block_res_sample=mid)
+
+
+class MultiControlNetModel(nn.Module):
+    """Several ControlNets whose residuals are summed in net order: diffusers 0.27.0 `MultiControlNetModel` as the
+    reference wraps a list of ControlNets (pipeline_PowerPaint_ControlNet.py:306; restated as recalled, not copied).
+    `forward` runs each net eagerly on the kernel path; the fused loop (`FusedDenoiser`) records all nets into one
+    step program instead."""
+
+    def __init__(self, controlnets):
+        super().__init__()
+        self.nets = nn.ModuleList(controlnets)
+
+    @property
+    def dtype(self) -> torch.dtype:
+        return self.nets[0].dtype
+
+    @property
+    def device(self) -> torch.device:
+        return self.nets[0].device
+
+    @torch.no_grad()
+    def forward(self, sample: torch.FloatTensor, timestep: Union[torch.Tensor, float, int],
+                encoder_hidden_states: torch.Tensor, controlnet_cond: List[torch.Tensor],
+                conditioning_scale: List[float], class_labels: Optional[torch.Tensor] = None,
+                timestep_cond: Optional[torch.Tensor] = None, attention_mask: Optional[torch.Tensor] = None,
+                added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
+                cross_attention_kwargs: Optional[Dict[str, Any]] = None, guess_mode: bool = False,
+                return_dict: bool = True):
+        """(down residuals, mid residual): the sum over nets, net 0 first. A tuple whatever `return_dict` says."""
+        down = mid = None
+        for i, (image, scale, net) in enumerate(zip(controlnet_cond, conditioning_scale, self.nets)):
+            d, m = net(sample, timestep, encoder_hidden_states, image, scale, class_labels=class_labels,
+                       timestep_cond=timestep_cond, attention_mask=attention_mask,
+                       added_cond_kwargs=added_cond_kwargs, cross_attention_kwargs=cross_attention_kwargs,
+                       guess_mode=guess_mode, return_dict=False)
+            if i == 0:
+                down, mid = d, m
+            else:
+                down = [a + b for a, b in zip(down, d)]
+                mid = mid + m
+        return down, mid

@@ -326,6 +326,22 @@ def tile_blend_desc(b: torch.Tensor, av: Optional[torch.Tensor], ah: Optional[to
     return Desc("tile_blend", d, (b, av, ah))
 
 
+def pool_broadcast_desc(x: torch.Tensor, out: torch.Tensor, prev: Optional[torch.Tensor] = None) -> Desc:
+    """out[s, p, c] = bf16(prev[s, p, c] + mean_p x[s, p, c]) over bf16 NHWC [batch, hw, channels] buffers
+    (include/powerpaint_b200.h, pp_pool_broadcast_desc): the global pooling of a side net's residual"""
+    for t, name in ((x, "x"), (out, "out"), (prev, "prev")):
+        if t is None:
+            continue
+        if t.dtype != BF16 or t.dim() != 3 or not t.is_cuda or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous CUDA bf16 [batch, hw, channels] tensor")
+        if t.shape != x.shape:
+            raise ValueError(f"{name} {tuple(t.shape)} does not match x {tuple(x.shape)}")
+    d = N.PoolBroadcastDesc()
+    d.x, d.prev, d.out = N.ptr(x), N.ptr(prev), N.ptr(out)
+    d.batch, d.hw, d.channels = x.shape
+    return Desc("pool_broadcast", d, (x, prev, out))
+
+
 class WindowList:
     """Windows (src_off, dst_off, src_row, dst_row, rows, cols) in elements of src / dst, checked against both
     tensors on the host and uploaded once; `channels` elements are copied per pixel, pixels src_pix / dst_pix
@@ -380,6 +396,8 @@ def run(desc: Desc) -> None:
         N.check(L.pp_solver_step(C.byref(desc.c), s), "pp_solver_step")
     elif desc.kind == "tile_blend":
         N.check(L.pp_tile_blend(C.byref(desc.c), s), "pp_tile_blend")
+    elif desc.kind == "pool_broadcast":
+        N.check(L.pp_pool_broadcast(C.byref(desc.c), s), "pp_pool_broadcast")
     else:
         raise ValueError(desc.kind)
 
@@ -509,7 +527,7 @@ class Program:
         fn = {"gemm": L.pp_program_add_gemm, "attn": L.pp_program_add_attention,
               "gn": L.pp_program_add_group_norm, "cfg_ddim": L.pp_program_add_cfg_ddim,
               "unipc": L.pp_program_add_unipc, "tile_blend": L.pp_program_add_tile_blend,
-              "solver": L.pp_program_add_solver_step}[desc.kind]
+              "solver": L.pp_program_add_solver_step, "pool_broadcast": L.pp_program_add_pool_broadcast}[desc.kind]
         N.check(fn(self._h, C.byref(desc.c)), f"pp_program_add_{desc.kind}")
         self._keep.append(desc.keep)
         self.labels.append(desc.kind)

@@ -214,8 +214,6 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         # valid for the reference, outside the hot path here
         if ip_adapter_image is not None or ip_adapter_image_embeds is not None:
             raise NotImplementedError("IP-adapter inputs are outside the hot path (unused by app.py)")
-        if guess_mode:
-            raise NotImplementedError("guess_mode is outside the hot path (unused by app.py)")
         if cross_attention_kwargs:
             raise NotImplementedError("cross_attention_kwargs (LoRA scale) is outside the hot path")
         self._guidance_scale = guidance_scale
@@ -228,6 +226,7 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
             batch_size = prompt_embeds.shape[0]
         device = self._execution_device
         do_cfg = self.do_classifier_free_guidance
+        guess_mode = guess_mode or self.brushnet.config.global_pool_conditions  # (:1240-1245)
         prompt_embeds = self._encode_prompt(promptA, promptB, tradoff, device, num_images_per_prompt, do_cfg,
                                             negative_promptA, negative_promptB, tradoff_nag,
                                             prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds)
@@ -236,9 +235,10 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         else:
             prompt_embedsU = prompt_embedsU.to(device=device, dtype=torch.float32)
         total = batch_size * num_images_per_prompt
-        image_t = self.prepare_image(image, width, height, total, num_images_per_prompt, device, torch.float32, do_cfg)
+        image_t = self.prepare_image(image, width, height, total, num_images_per_prompt, device, torch.float32, do_cfg,
+                                     guess_mode)
         original_mask = self.prepare_image(mask, width, height, total, num_images_per_prompt, device, torch.float32,
-                                           do_cfg)
+                                           do_cfg, guess_mode)
         original_mask = (original_mask.sum(1)[:, None, :, :] < 0).to(image_t.dtype)
         height, width = image_t.shape[-2:]
         if timesteps is not None:
@@ -266,8 +266,9 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         else:
             noise = latents.to(device)
         latents = noise * self.scheduler.init_noise_sigma
-        # global RNG, 2B batch under CFG — exactly as the reference (:1338-1341)
-        if do_cfg and hasattr(self.vae, "decode_postprocessed"):
+        # global RNG, 2B batch under CFG (B in guess mode, whose images are not doubled) — exactly as the reference
+        # (:1338-1341)
+        if do_cfg and not guess_mode and hasattr(self.vae, "decode_postprocessed"):
             # both CFG halves hold the same images: encode them once and duplicate the moments; the noise is still
             # drawn for all 2B samples in one call, so the RNG stream equals the reference's
             dist = self.vae.encode(image_t[:total]).latent_dist
@@ -317,14 +318,16 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
                 if callback is not None and i % (callback_steps or 1) == 0:
                     callback(i, t, lat)
                 return new
-        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
-        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
+        # `scoef` / `guess_mode` are passed only when set: a denoiser whose `run` predates them keeps serving DDIM
+        # and UniPC unchanged
+        opt = {} if scoef is None else dict(scoef=scoef)
+        if guess_mode:
+            opt["guess_mode"] = True
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds,
                                       timesteps=ts, coef=coef, guidance_scale=guidance_scale,
                                       extra=conditioning_latents, side_scale=float(brushnet_conditioning_scale),
                                       side_keep=keep, ucoef=ucoef,
-                                      noise_fn=noise_fn, callback=cb,
-                                      **({} if scoef is None else dict(scoef=scoef)))
+                                      noise_fn=noise_fn, callback=cb, **opt)
         if finish is not None:
             finish()
         image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)

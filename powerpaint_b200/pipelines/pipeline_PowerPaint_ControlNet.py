@@ -5,21 +5,26 @@ The loop (:1663-1735: ControlNet on the 4-channel latents + control image, 9-cha
 (`FusedDenoiser(mode="controlnet")`); the t-independent `controlnet_cond_embedding(control_image)`
 is evaluated once per call instead of once per step (SURVEY.md App. C (3)).
 
-Out of scope like upstream's dead code: `predict_woControl` (:996-1345, a buggy copy of the v1
-`__call__`), MultiControlNet, guess_mode.
+Several ControlNets (a list, wrapped in `MultiControlNetModel` as :306 does), `guess_mode` and pooled
+(`global_pool_conditions`) ControlNets run on the same fused loop (see `powerpaint_b200.denoise`).
+
+Out of scope like upstream's dead code: `predict_woControl` (:996-1345, a buggy copy of the v1 `__call__`).
 """
 from __future__ import annotations
 
+import logging
 from typing import Callable, List, Optional, Union
 
 import torch
 
 from ..denoise import FusedDenoiser
-from ..models.unet_2d_condition import ControlNetModel, UNet2DConditionModel
+from ..models.unet_2d_condition import ControlNetModel, MultiControlNetModel, UNet2DConditionModel
 from .common import (StableDiffusionPipelineOutput, check_control_guidance, check_image, check_prompt_arguments,
                      decode_latents, prepare_mask_and_masked_image, preprocess_image, randn_tensor,
                      solver_loop_inputs, uint8_device_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
+
+logger = logging.getLogger(__name__)
 
 
 class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
@@ -28,13 +33,14 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         super().__init__(vae, text_encoder, tokenizer, unet, scheduler, safety_checker, feature_extractor,
                          requires_safety_checker)
         if isinstance(controlnet, (list, tuple)):
-            raise NotImplementedError("MultiControlNet is outside the hot path")
+            controlnet = MultiControlNetModel(controlnet)
         self.controlnet = controlnet
         self._denoiser_side = None
 
     def denoiser(self) -> FusedDenoiser:
-        if not isinstance(self.unet, UNet2DConditionModel) or not isinstance(self.controlnet, ControlNetModel):
-            assert False, "unet / controlnet must be powerpaint_b200 UNet2DConditionModel / ControlNetModel"
+        nets = self.controlnet.nets if isinstance(self.controlnet, MultiControlNetModel) else [self.controlnet]
+        if not isinstance(self.unet, UNet2DConditionModel) or not all(isinstance(n, ControlNetModel) for n in nets):
+            assert False, "unet / controlnet must be powerpaint_b200 UNet2DConditionModel / ControlNetModel(s)"
         if self._denoiser is None or self._denoiser_unet is not self.unet or self._denoiser_side is not self.controlnet:
             self._denoiser = FusedDenoiser(self.unet, self.controlnet, mode="controlnet")
             self._denoiser_unet, self._denoiser_side = self.unet, self.controlnet
@@ -51,11 +57,41 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps} of type"
                              f" {type(callback_steps)}.")
         check_prompt_arguments(prompt, negative_prompt, prompt_embeds, negative_prompt_embeds)
-        if not isinstance(self.controlnet, ControlNetModel):
+        multi = isinstance(self.controlnet, MultiControlNetModel)
+        if multi and isinstance(prompt, list):
+            logger.warning(f"You have {len(self.controlnet.nets)} ControlNets and you have passed {len(prompt)}"
+                           " prompts. The conditionings will be fixed across the prompts.")
+        if isinstance(self.controlnet, ControlNetModel):
+            check_image(image, prompt, prompt_embeds)
+        elif multi:
+            if not isinstance(image, list):
+                raise TypeError("For multiple controlnets: `image` must be type `list`")
+            elif any(isinstance(i, list) for i in image):
+                raise ValueError("A single batch of multiple conditionings are supported at the moment.")
+            elif len(image) != len(self.controlnet.nets):
+                raise ValueError("For multiple controlnets: `image` must have the same length as the number of "
+                                 f"controlnets, but got {len(image)} images and {len(self.controlnet.nets)} "
+                                 "ControlNets.")
+            for image_ in image:
+                check_image(image_, prompt, prompt_embeds)
+        else:
             assert False
-        check_image(image, prompt, prompt_embeds)
-        if not isinstance(controlnet_conditioning_scale, float):
-            raise TypeError("For single controlnet: `controlnet_conditioning_scale` must be type `float`.")
+        if isinstance(self.controlnet, ControlNetModel):
+            if not isinstance(controlnet_conditioning_scale, float):
+                raise TypeError("For single controlnet: `controlnet_conditioning_scale` must be type `float`.")
+        elif isinstance(controlnet_conditioning_scale, list):
+            # the reference's length check sits in an `elif` its `if` always shadows, so a scale list of the wrong
+            # length passes here (and `zip` later drops the nets it has no scale for)
+            if any(isinstance(i, list) for i in controlnet_conditioning_scale):
+                raise ValueError("A single batch of multiple conditionings are supported at the moment.")
+        if len(control_guidance_start) != len(control_guidance_end):
+            raise ValueError(f"`control_guidance_start` has {len(control_guidance_start)} elements, but "
+                             f"`control_guidance_end` has {len(control_guidance_end)} elements. Make sure to provide "
+                             "the same number of elements to each list.")
+        if multi and len(control_guidance_start) != len(self.controlnet.nets):
+            n = len(self.controlnet.nets)
+            raise ValueError(f"`control_guidance_start`: {control_guidance_start} has {len(control_guidance_start)} "
+                             f"elements but there are {n} controlnets available. Make sure to provide {n}.")
         check_control_guidance(control_guidance_start, control_guidance_end)
 
     def check_image(self, image, prompt, prompt_embeds):
@@ -106,13 +142,12 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         elif not isinstance(control_guidance_end, list) and isinstance(control_guidance_start, list):
             control_guidance_end = len(control_guidance_start) * [control_guidance_end]
         elif not isinstance(control_guidance_start, list) and not isinstance(control_guidance_end, list):
-            control_guidance_start, control_guidance_end = [control_guidance_start], [control_guidance_end]
+            mult = len(self.controlnet.nets) if isinstance(self.controlnet, MultiControlNetModel) else 1
+            control_guidance_start, control_guidance_end = mult * [control_guidance_start], mult * [control_guidance_end]
         self.check_inputs_controlnet(prompt, control_image, height, width, callback_steps, negative_prompt,
                                      prompt_embeds, negative_prompt_embeds, controlnet_conditioning_scale,
                                      control_guidance_start, control_guidance_end)
         # valid for the reference, outside the hot path here
-        if guess_mode:
-            raise NotImplementedError("guess_mode is outside the hot path")
         if cross_attention_kwargs:
             raise NotImplementedError("cross_attention_kwargs (LoRA scale) is outside the hot path")
         if prompt is not None and isinstance(prompt, str):
@@ -123,12 +158,17 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             batch_size = prompt_embeds.shape[0]
         device = self._execution_device
         do_cfg = guidance_scale > 1.0
+        nets = self.controlnet.nets if isinstance(self.controlnet, MultiControlNetModel) else [self.controlnet]
+        multi = isinstance(self.controlnet, MultiControlNetModel)
+        if multi and isinstance(controlnet_conditioning_scale, float):  # (:1533-1534)
+            controlnet_conditioning_scale = [controlnet_conditioning_scale] * len(nets)
+        guess_mode = guess_mode or nets[0].config.global_pool_conditions  # (:1536-1541)
         prompt_embeds = self._encode_prompt(promptA, promptB, tradoff, device, num_images_per_prompt, do_cfg,
                                             negative_promptA, negative_promptB, tradoff_nag,
                                             prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds)
         total = batch_size * num_images_per_prompt
-        control = self.prepare_control_image(control_image, width, height, total, num_images_per_prompt, device,
-                                             torch.float32, do_cfg)
+        control = [self.prepare_control_image(ci, width, height, total, num_images_per_prompt, device, torch.float32,
+                                              do_cfg, guess_mode) for ci in (control_image if multi else [control_image])]
         if uint8_device_inputs(self.vae, image, mask):  # see StableDiffusionInpaintPipeline.__call__
             if image.shape[-2:] != mask.shape[-2:] or image.shape[0] != mask.shape[0] or mask.shape[1] != 1:
                 raise ValueError("uint8 image [B,3,H,W] and mask [B,1,H,W] must agree in batch and size")
@@ -154,8 +194,8 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         mask, masked_image_latents = self.prepare_mask_latents(mask, masked_image, total, height, width, torch.float32,
                                                                device, generator, do_cfg)
         extra_step_kwargs = self.prepare_extra_step_kwargs(generator, eta)
-        keep = [1.0 - float(i / len(timesteps) < control_guidance_start[0]
-                            or (i + 1) / len(timesteps) > control_guidance_end[0]) for i in range(len(timesteps))]
+        keeps = [[1.0 - float(i / len(timesteps) < s or (i + 1) / len(timesteps) > e) for i in range(len(timesteps))]
+                 for s, e in zip(control_guidance_start, control_guidance_end)]
         # `controlnet_keep` (ref:pipeline_PowerPaint_ControlNet.py:1652-1658): the per-step scale
         # conditioning_scale * keep[i] sits in the device coefficient table the recorded program indexes
         coef = self.scheduler.step_coefficients(timesteps, eta=extra_step_kwargs.get("eta", 0.0))
@@ -178,15 +218,24 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
                 if i % callback_steps == 0:
                     callback(i, t, lat)
                 return None
-        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
-        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
+        if multi:
+            # `MultiControlNetModel` zips nets with scales: a net without a scale adds nothing (a zero scale)
+            scales = [float(v) for v in controlnet_conditioning_scale][:len(nets)]
+            side = dict(control_image=control, side_scale=scales + [0.0] * (len(nets) - len(scales)), side_keep=keeps)
+        else:
+            scale = controlnet_conditioning_scale
+            side = dict(control_image=control[0], side_scale=float(scale[0] if isinstance(scale, list) else scale),
+                        side_keep=keeps[0])
+        # `guess_mode` / `scoef` are passed only when set: a denoiser whose `run` predates them keeps serving the
+        # plain single-ControlNet call unchanged
+        if guess_mode:
+            side["guess_mode"] = True
+        if scoef is not None:
+            side["scoef"] = scoef
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds,
-                                      control_image=control, timesteps=timesteps, coef=coef,
-                                      guidance_scale=guidance_scale,
+                                      timesteps=timesteps, coef=coef, guidance_scale=guidance_scale,
                                       extra=torch.cat([mask, masked_image_latents], dim=1),
-                                      side_scale=float(controlnet_conditioning_scale), side_keep=keep,
-                                      noise_fn=noise_fn, ucoef=ucoef, callback=cb,
-                                      **({} if scoef is None else dict(scoef=scoef)))
+                                      noise_fn=noise_fn, ucoef=ucoef, callback=cb, **side)
         if finish is not None:
             finish()
         image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
