@@ -12,11 +12,13 @@
 //               in shared memory) into registers; online softmax in fp32 registers (exp2 domain; a row lives in
 //               the four lanes of a quad, so row max / sum need two shuffles); P rounded to fp16 / bf16 stays in
 //               registers and is the A operand of O += P V (wgmma with A from registers, V^T from shared memory,
-//               O in registers). The two warpgroups run independently, so one's softmax overlaps the other's MMAs.
-// The row sums add the 16-bit P the MMA actually sees. Head dims that are not multiples of 64/16 need no
+//               O in registers). DV <= 64: the warpgroups take turns on the tensor cores and each issues S of the
+//               next key block with PV of this one, so the exponentials overlap MMAs; DV > 64: they run independently.
+// The row sums add the 16-bit P the MMA actually sees (DV <= 64 with d < DV: the PV MMA adds them up itself, in
+// column d, against a row of ones in V^T). Head dims that are not multiples of 64/16 need no
 // padding in HBM: the Q/K tensor maps are (d, heads, tokens, batch) so TMA zero-fills channels >= d of each head,
 // and V is consumed transposed ([batch, heads*d, keys], keys contiguous; produced by the projection GEMM's
-// transposed epilogue) so both MMAs read K-major SWIZZLE_128B operands; V^T rows >= d read as zeros.
+// transposed epilogue) so both MMAs read K-major SWIZZLE_128B operands; V^T rows >= d read as zeros (DV > 64).
 #include <math.h>
 
 #include <algorithm>
@@ -38,6 +40,14 @@ __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
+}
+
+// named barriers of `nthreads` threads (multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // DV: width of the PV product (head dim rounded up to one of the instantiated widths)
@@ -96,6 +106,22 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
         }
         fence_mbar_init();
     }
+    if constexpr (DCH == 1) {
+        // d < DV: the V^T box has d rows, and rows d .. DV - 1 of both chunks of every stage are written here, once:
+        // row d is 1.0 in the P type, the rest 0. Column d of O then accumulates the row sum of P. A row of equal
+        // 16-byte units is the same under the 128-byte swizzle, and TMA never writes outside its box.
+        if (p.d < DV) {
+            const uint32_t one2 = F16 ? 0x3C003C00u : 0x3F803F80u;
+            const int rows = DV - p.d;
+            for (int i = threadIdx.x; i < 2 * S * rows * 8; i += ATT_THREADS) {  // 8 16-byte units per 128-byte row
+                const int r = (i >> 3) % rows, chunk = (i >> 3) / rows;
+                const uint32_t v = r == 0 ? one2 : 0u;
+                *reinterpret_cast<uint4*>(smem_raw + (sV0 - raw) + chunk * V_CHUNK + (p.d + r) * 128 + (i & 7) * 16) =
+                    make_uint4(v, v, v, v);
+            }
+            fence_proxy_async_smem();  // the tensor cores read these rows through the async proxy
+        }
+    }
     __syncthreads();
     pdl_wait();  // Q / K / V^T come from the preceding kernels
     pdl_launch_dependents();
@@ -111,7 +137,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
                 const int s = j % S;
                 const uint32_t ph = (j / S) & 1;
                 mbar_wait(bar_kv_empty(s), ph ^ 1u);
-                mbar_arrive_expect_tx(bar_kv_full(s), DCH * ATT_CHUNK_BYTES + V_STAGE);
+                if constexpr (DCH == 1) mbar_arrive_expect_tx(bar_kv_full(s), ATT_CHUNK_BYTES + 256u * p.d);  // V^T: d rows
+                else mbar_arrive_expect_tx(bar_kv_full(s), DCH * ATT_CHUNK_BYTES + V_STAGE);
                 const uint32_t dK = sK0 + s * DCH * ATT_CHUNK_BYTES;
                 const uint32_t dV = sV0 + s * V_STAGE;
 #pragma unroll
@@ -119,6 +146,200 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_c
                     tma_load_4d(dK + dc * ATT_CHUNK_BYTES, &p.tmK, bar_kv_full(s), dc * 64, head, j * ATT_BN, b);
                 tma_load_3d(dV, &p.tmV, bar_kv_full(s), j * ATT_BN, 0, b * p.heads + head);
                 tma_load_3d(dV + V_CHUNK, &p.tmV, bar_kv_full(s), j * ATT_BN + 64, 0, b * p.heads + head);
+            }
+        }
+    } else if constexpr (DCH == 1) {
+        // ============ consumer warpgroups, DV <= 64: tensor-core turns and look-ahead ============
+        // At these widths the exponentials (MUFU) bound the block, not the MMAs, so the MMAs are hidden under them:
+        //  - turns: a warpgroup issues its MMAs only in its turn (named barrier 1 + wg) and then hands the turn to the
+        //    other warpgroup, so one warpgroup's softmax runs while the other's MMAs run;
+        //  - look-ahead: S(j+1) = Q K(j+1)^T and O += P(j) V(j) are issued as two commit groups, and the max and the
+        //    exponentials of S(j+1) run while PV(j) is still on the tensor cores. A warp therefore holds stage j + 1
+        //    before it releases stage j, which needs a ring of two stages or more.
+        // The arithmetic is the one of the DV > 64 loop below, operation for operation, except for the row sums when
+        // d < DV: the tensor cores add them up in column d of O (V^T row d is all ones), which the rescale of O by
+        // alpha rescales too. They add the same 16-bit P the MMA multiplies.
+        static_assert(S >= 2, "the look-ahead holds two ring stages at once");
+        const int wg = warp >> 2, w4 = warp & 3;
+        const int lane = (int)lane_id();
+        const int qc = 2 * (lane & 3);  // first of the two columns this thread holds in each 8-column group
+        const float c = p.scale_log2;
+        const bool sum_in_o = p.d < DV;
+        // turn barriers: both warpgroups (256 threads) meet on each; warpgroup wg waits on 1 + wg, arrives on 2 - wg
+        const int turn_mine = 1 + wg, turn_other = 2 - wg;
+        float o[DV / 2];
+#pragma unroll
+        for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
+        float m_run0 = -INFINITY, m_run1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+        float sc[64];    // S of the newest key block, then its exponentials
+        uint32_t pa[32];  // P of the block whose PV product is next, in the A-operand layout of the k16 slices
+        const uint32_t zero = (uint32_t)p.nk >> 31;  // nk > 0, so 0, but not a constant to the compiler
+        const uint32_t qa = sQ + wg * (ATT_CHUNK_BYTES / 2);
+        // S = Q K(j)^T into sc. Every wgmma count is a compile-time constant and no wgmma sits under a runtime
+        // condition: that would make ptxas serialise all of them (C7519).
+        auto issue_s = [&](int j) {
+            const uint32_t kb = sK0 + (j % S) * ATT_CHUNK_BYTES;
+#pragma unroll
+            for (int ks = 0; ks < DV / 16; ++ks)
+                Wgmma<ATT_BN>::ss_bf16(sc, wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(qa), ks * 16),
+                                       wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(kb), ks * 16), 1);
+            wgmma_commit();
+        };
+        // O += P(j) V(j), all 8 k-steps of 16 keys: keys past the end have P = 0
+        auto issue_pv = [&](int j) {
+            const uint32_t vb = sV0 + (j % S) * V_STAGE;
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) {
+                const uint64_t db = wgmma_desc_advance_k(wgmma_desc_kmajor_sw128(vb + (ks >> 2) * V_CHUNK), (ks & 3) * 16);
+                const uint32_t(&a)[4] = *reinterpret_cast<const uint32_t(*)[4]>(&pa[4 * ks]);
+                if constexpr (F16) Wgmma<DV>::rs_f16(o, a, db, 1);
+                else Wgmma<DV>::rs_bf16(o, a, db, 1);
+            }
+            wgmma_commit();
+        };
+        // masks and exponentiates sc (key block j) in place; returns the factors O and l are rescaled by
+        auto softmax = [&](int j, float& al0, float& al1) {
+            const int nvalid = min(ATT_BN, p.nk - j * ATT_BN);
+            if (nvalid < ATT_BN) {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    if (8 * i + qc >= nvalid) sc[4 * i] = sc[4 * i + 2] = -INFINITY;
+                    if (8 * i + qc + 1 >= nvalid) sc[4 * i + 1] = sc[4 * i + 3] = -INFINITY;
+                }
+            }
+            float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                mx0 = fmaxf(mx0, fmaxf(sc[4 * i], sc[4 * i + 1]));
+                mx1 = fmaxf(mx1, fmaxf(sc[4 * i + 2], sc[4 * i + 3]));
+            }
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+            const float mn0 = fmaxf(m_run0, mx0 * c), mn1 = fmaxf(m_run1, mx1 * c);
+            al0 = fast_exp2(m_run0 - mn0);
+            al1 = fast_exp2(m_run1 - mn1);
+            m_run0 = mn0;
+            m_run1 = mn1;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                sc[4 * i] = fast_exp2(fmaf(sc[4 * i], c, -mn0));
+                sc[4 * i + 1] = fast_exp2(fmaf(sc[4 * i + 1], c, -mn0));
+                sc[4 * i + 2] = fast_exp2(fmaf(sc[4 * i + 2], c, -mn1));
+                sc[4 * i + 3] = fast_exp2(fmaf(sc[4 * i + 3], c, -mn1));
+            }
+        };
+        // after PV(j) has retired: rescale O and l, round the exponentials to P(j + 1)
+        auto rescale_and_pack = [&](float al0, float al1) {
+            l0 *= al0;
+            l1 *= al1;
+#pragma unroll
+            for (int i = 0; i < DV / 8; ++i) {
+                o[4 * i] *= al0; o[4 * i + 1] *= al0;
+                o[4 * i + 2] *= al1; o[4 * i + 3] *= al1;
+            }
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                pa[2 * i] = pack_p<F16>(sc[4 * i], sc[4 * i + 1]);
+                pa[2 * i + 1] = pack_p<F16>(sc[4 * i + 2], sc[4 * i + 3]);
+            }
+            if (!sum_in_o) {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    l0 += sum_p<F16>(pa[2 * i]);
+                    l1 += sum_p<F16>(pa[2 * i + 1]);
+                }
+            }
+        };
+        float al0, al1;
+        if (wg == 1) named_bar_arrive(turn_other, 256);  // warpgroup 0 takes the first turn
+        mbar_wait(bar_q, 0);
+        {
+            const int j = 0, s = 0;
+            mbar_wait(bar_kv_full(s), (j / S) & 1);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) sc[i] = 0.f;
+            named_bar_sync(turn_mine, 256);
+            wgmma_fence();
+            issue_s(j);
+            named_bar_arrive(turn_other, 256);
+            wgmma_wait<0>();
+            wgmma_fence_regs(sc);
+            softmax(j, al0, al1);
+            rescale_and_pack(al0, al1);
+        }
+        for (int j = 0; j + 1 < nkv; ++j) {
+            const int s = j % S, s1 = (j + 1) % S;
+            mbar_wait(bar_kv_full(s1), ((j + 1) / S) & 1);  // hold stage j + 1 ...
+#pragma unroll
+            for (int i = 0; i < 64; ++i) sc[i] = 0.f;
+            named_bar_sync(turn_mine, 256);
+            wgmma_fence();
+            issue_s(j + 1);
+            issue_pv(j);
+            named_bar_arrive(turn_other, 256);
+            wgmma_wait<1>();  // S(j + 1) has landed; PV(j) may still run
+            wgmma_fence_regs(sc);
+            softmax(j + 1, al0, al1);
+            // The exponentials are what overlaps PV(j), so they must stay ahead of the wait, but ptxas would start
+            // their block with the wait, and sinks them past any branch whose other side does not read them. This
+            // branch never runs (zero is 0); its use of every exponential pins them above the wait.
+            if (zero) {
+                float t = 0.f;
+#pragma unroll
+                for (int i = 0; i < 64; ++i) t += sc[i];
+                p.out[0] = __float2bfloat16(t);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
+            wgmma_fence_regs(pa);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_kv_empty(s));  // ... then release stage j
+            rescale_and_pack(al0, al1);
+        }
+        {
+            const int s = (nkv - 1) % S;
+            named_bar_sync(turn_mine, 256);
+            wgmma_fence();
+            issue_pv(nkv - 1);
+            if (wg == 0) named_bar_arrive(turn_other, 256);  // the last turn is warpgroup 1's: nothing left pending
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
+            wgmma_fence_regs(pa);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_kv_empty(s));
+        }
+        // epilogue: O / l -> bf16
+        if (sum_in_o) {
+            // column d (a multiple of 8) is element 4 (d / 8) (+ 2 for the second row) of the quad's first lane;
+            // selected with constant register indices, so O stays in registers
+            const int di = p.d >> 3;
+#pragma unroll
+            for (int i = 0; i < DV / 8; ++i) {
+                if (i == di) {
+                    l0 = o[4 * i];
+                    l1 = o[4 * i + 2];
+                }
+            }
+            l0 = __shfl_sync(0xffffffffu, l0, lane & ~3);
+            l1 = __shfl_sync(0xffffffffu, l1, lane & ~3);
+        } else {
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+        }
+        const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+        const int qi0 = q0 + 64 * wg + 16 * w4 + (lane >> 2), qi1 = qi0 + 8;
+        __nv_bfloat16* orow0 = p.out + ((int64_t)b * p.nq + qi0) * p.o_ld + head * p.d;
+        __nv_bfloat16* orow1 = orow0 + 8 * p.o_ld;
+#pragma unroll
+        for (int i = 0; i < DV / 8; ++i) {
+            const int col = 8 * i + qc;  // d % 8 == 0: col < d implies col + 1 < d
+            if (col < p.d) {
+                if (qi0 < p.nq) *reinterpret_cast<uint32_t*>(orow0 + col) = pack_bf16x2(o[4 * i] * inv0, o[4 * i + 1] * inv0);
+                if (qi1 < p.nq) *reinterpret_cast<uint32_t*>(orow1 + col) = pack_bf16x2(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
             }
         }
     } else {
@@ -325,10 +546,11 @@ int attn_prepare(const pp_attn_desc& d, AttnLaunch* out) {
         if (rc) return rc;
     }
     {
-        // rows d .. dv - 1 of the box lie outside the head: TMA zero-fills them
+        // dv > 64: rows d .. dv - 1 of the box lie outside the head, TMA zero-fills them. dv <= 64: the box has d rows,
+        // the kernel writes the rows past it itself (the row-sum row)
         uint64_t dims[3] = {(uint64_t)d.nk, (uint64_t)d.d, (uint64_t)d.batch * d.heads};
         uint64_t str[2] = {(uint64_t)d.vt_ld * 2, (uint64_t)d.vt_ld * 2 * d.d};
-        uint32_t box[3] = {64, (uint32_t)p.dv, 1};
+        uint32_t box[3] = {64, (uint32_t)(p.dv <= 64 ? d.d : p.dv), 1};
         int rc = make_tmap_bf16(&p.tmV, d.vt, 3, dims, str, box, true);
         if (rc) return rc;
     }
