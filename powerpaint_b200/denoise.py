@@ -46,7 +46,7 @@ from typing import Callable, Optional
 import torch
 
 from . import ops
-from .engine import NetEngine, Plan, guess_mode_alphas
+from .engine import NetEngine, Pool, SideOutputs, guess_mode_alphas, lru_get
 
 MAX_STEPS = 1000
 X_IN_C = 16
@@ -82,20 +82,18 @@ class FusedDenoiser:
     # ------------------------------------------------------------------ plan
     def _get(self, B: int, h: int, w: int, do_cfg: bool, ctx_len: int, with_noise: bool,
              extra_per_copy: bool, sched: str = "ddim", blend: bool = False, guess: bool = False) -> dict:
-        K = len(self.sides)
         pools = tuple(bool(getattr(s.config, "global_pool_conditions", False)) for s in self.sides)
         # the key carries the parameter generation of each model: `load_state_dict` / `.to()` invalidate it,
         # and the cached entry keeps its engines alive, so a recycled id() can never alias a stale program
-        key = (B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, K, guess, pools,
+        key = (B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, len(self.sides), guess, pools,
                self.unet.generation, tuple(s.generation for s in self.sides))
-        st = self._cache.get(key)
-        if st is not None:
-            self._cache.move_to_end(key)
-            return st
         for k in [k for k in self._cache if k[-2:] != key[-2:]]:  # (unet generation, side generations)
             del self._cache[k]  # plans recorded against replaced weights
-        while len(self._cache) >= self.MAX_PLANS:
-            self._cache.popitem(last=False)
+        return lru_get(self._cache, key, self.MAX_PLANS, lambda: self._record(
+            B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools))
+
+    def _record(self, B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools) -> dict:
+        K = len(self.sides)
         dev = self.unet.device
         nb = 2 * B if do_cfg else B
         ns = B if guess and do_cfg else nb  # rows the side nets run on: the conditional half in guess mode
@@ -106,56 +104,30 @@ class FusedDenoiser:
         step_idx = torch.zeros(1, dtype=torch.int32, device=dev)
         coef = torch.zeros(MAX_STEPS, 8, dtype=torch.float32, device=dev)
         side_scale = torch.zeros(MAX_STEPS, max(K, 1), dtype=torch.float32, device=dev)  # scale x keep per step, net
-        pool = Plan()  # the nets of one step share one activation pool
-        shared = dict(program=prog, ctx_program=ctxprog, x_in=x_in, timesteps=timesteps, step_idx=step_idx, pool=pool)
+        pool = Pool(dev)  # the nets of one step share one activation pool
+        common = dict(pool=pool, program=prog, ctx_program=ctxprog, steps=(timesteps, step_idx))
         st = dict(B=B, nb=nb, ns=ns, h=h, w=w, do_cfg=do_cfg, x_in=x_in, timesteps=timesteps, step_idx=step_idx,
                   coef=coef, side_scale=side_scale, program=prog, ctx_program=ctxprog, graph=False,
                   with_noise=with_noise, extra_per_copy=extra_per_copy,
                   engines=(ue,) + tuple(s.engine() for s in self.sides))
         side_x = x_in[nb - ns:]  # contiguous: the CFG halves are stacked [uncond; cond]
         down_s, mid_s, up_s = ue._state_shapes(nb, h, w)
-
-        def residuals(shapes):  # 2B-row buffers the UNet reads; rows the side nets never write stay zero
-            return [torch.zeros(nb, hh * ww, c, dtype=torch.bfloat16, device=dev) for (c, hh, ww) in shapes]
-
-        def rows(bufs):  # the rows the side nets write
-            return [b[nb - ns:].reshape(-1, b.shape[-1]) for b in bufs]
-
-        def side_shared(k):
-            return dict(shared, x_in=side_x, scale_dev=(side_scale[:, k], step_idx, K))
-
+        nd = len(down_s)
+        # 2B-row residual buffers the UNet reads, in residual order; rows the side nets never write stay zero
+        shapes = {"v1": [], "brushnet": down_s + [mid_s] + up_s, "controlnet": down_s + [mid_s]}[self.mode]
+        res = [pool.tensor(nb, hh * ww, c, zero=True) for (c, hh, ww) in shapes]
         side_plans = []
-        res_bytes = 0
-        if self.mode == "brushnet":
-            se: NetEngine = self.sides[0].engine()
-            side_plan = se._build_plan(ns, h, w, ctx_len, False, False, True, 0, shared=side_shared(0))
-            adds_d, add_m, adds_u = residuals(down_s), residuals([mid_s])[0], residuals(up_s)
-            res_bytes = sum(t.numel() * 2 for t in adds_d + [add_m] + adds_u)
-            alphas = guess_mode_alphas(len(adds_d) + 1 + len(adds_u)) if guess and not pools[0] else None
-            se.append_brushnet_outputs(side_plan, 1.0, targets=(rows(adds_d), rows([add_m])[0], rows(adds_u)),
-                                       scale_dev=(side_scale[:, 0], step_idx, K), alphas=alphas, pool=pools[0])
-            side_plans.append(side_plan)
-            uplan = ue._build_plan(nb, h, w, ctx_len, True, False, True, 0, shared=dict(shared, adds=(adds_d, add_m, adds_u)))
-            st["residuals"] = adds_d + [add_m] + adds_u
-        elif self.mode == "controlnet":
-            cn_d, cn_m = residuals(down_s), residuals([mid_s])[0]
-            res_bytes = sum(t.numel() * 2 for t in cn_d + [cn_m])
-            prev = None
-            for k, net in enumerate(self.sides):
-                last = k == K - 1
-                alphas = guess_mode_alphas(len(cn_d) + 1) if guess and not pools[k] else None
-                sp = net.engine()._build_plan(ns, h, w, ctx_len, False, False, True, 0,
-                                              shared=dict(side_shared(k), side_alphas=alphas, side_pool=pools[k],
-                                                          side_targets=(rows(cn_d), rows([cn_m])[0]) if last else None,
-                                                          side_prev=prev))
-                prev = (sp.outputs["down"], sp.outputs["mid"])
-                side_plans.append(sp)
-            uplan = ue._build_plan(nb, h, w, ctx_len, False, True, True, 0, shared=dict(shared, cn=(cn_d, cn_m)))
-            st["residuals"] = cn_d + [cn_m]
-        else:
-            uplan = ue._build_plan(nb, h, w, ctx_len, False, False, True, 0, shared=shared)
-        st["uplan"], st["side_plans"] = uplan, side_plans
-        st["side_plan"] = side_plans[0] if side_plans else None
+        for k, net in enumerate(self.sides):  # in net order; the last one writes the side-net rows of `res`
+            prev = side_plans[-1].outputs["down"] + [side_plans[-1].outputs["mid"]] if side_plans else None
+            side = SideOutputs(scale=(side_scale[:, k], step_idx, K),
+                               alphas=guess_mode_alphas(len(res)) if guess and not pools[k] else None,
+                               global_pool=pools[k], prev=prev,
+                               targets=[b[nb - ns:].reshape(-1, b.shape[-1]) for b in res] if k == K - 1 else None)
+            side_plans.append(net.engine()._build_plan(ns, h, w, ctx_len, x_in=side_x, side=side, **common))
+        uplan = ue._build_plan(nb, h, w, ctx_len, x_in=x_in, **common,
+                               adds=(res[:nd], res[nd], res[nd + 1:]) if self.mode == "brushnet" else None,
+                               cn=(res[:nd], res[nd]) if self.mode == "controlnet" else None)
+        st["uplan"], st["side_plans"], st["residuals"] = uplan, side_plans, res
         # fp32 master latents and the constant channels (channels-last)
         n_extra = nb if extra_per_copy else B
         st["latents"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
@@ -190,8 +162,7 @@ class FusedDenoiser:
                                        next_c=X_IN_C, n_copies=2 if do_cfg else 1, extra=None, extra_c=0,
                                        blend_x0=st.get("blend_x0"), blend_mask=st.get("blend_mask"),
                                        blend_noise=st.get("blend_noise")))
-        st["bytes"] = uplan.bytes + sum(p.bytes for p in side_plans) + res_bytes
-        self._cache[key] = st
+        st["bytes"] = pool.bytes
         return st
 
     @property

@@ -34,7 +34,7 @@ import torch.nn as nn
 
 from .. import _native as N
 from .. import ops
-from ..engine import BF16, NetEngine, Plan, _ceil
+from ..engine import BF16, Plan, Pool, Recorder, _ceil
 
 
 # --------------------------------------------------------------------------- parameter layout
@@ -183,41 +183,13 @@ def vae_tile_geometry(encode: bool, h: int, w: int, tile_sample_min_size: int, t
 
 
 # --------------------------------------------------------------------------- engine
-class VaeEngine(NetEngine):
+class VaeEngine(Recorder):
     """Records VAE encode / decode as `pp_program`s over the conv / GroupNorm / GEMM kernels of the denoising
-    step (buffer recycling, epilogue GroupNorm statistics and weight packing are inherited from `NetEngine`)."""
+    step (buffer recycling, epilogue GroupNorm statistics, weight packing and the resnet are `Recorder`'s)."""
 
     GN_EPS = 1e-6
-    MAX_PLANS = 2
-
-    def __init__(self, cfg: SimpleNamespace, state_dict: Dict[str, torch.Tensor], device):
-        self.cfg = cfg  # needs .norm_num_groups for _gn
-        self.kind = "vae"
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("VaeEngine needs a CUDA device: there is no CPU path")
-        N.lib()
-        self._sd = state_dict
-        self._w: Dict[str, torch.Tensor] = {}
-        self._plans: "OrderedDict[tuple, Plan]" = OrderedDict()
 
     # ---- blocks
-    def _vae_resnet(self, plan, prog, name, x, nb, h, w, cout):
-        hw = h * w
-        cin = x.shape[-1]
-        n1 = self._gn(plan, prog, x, None, nb, hw, name + ".norm1", self.GN_EPS, True)
-        t1 = self._conv3(plan, prog, n1, nb, h, w, name + ".conv1", cout, stats=True)
-        self._free(plan, n1)
-        n2 = self._gn(plan, prog, t1, None, nb, hw, name + ".norm2", self.GN_EPS, True)
-        self._free(plan, t1)
-        sc, owned = x, None
-        if cin != cout:
-            sc = owned = self._linear(plan, prog, x, nb * hw, name + ".conv_shortcut", cout,
-                                      bias=self.vec(name + ".conv_shortcut.bias"))
-        out = self._conv3(plan, prog, n2, nb, h, w, name + ".conv2", cout, res1=sc, stats=True)
-        self._free(plan, n2, owned)
-        return out
-
     def _vae_attention(self, plan, prog, name, x, nb, h, w):
         """one head over all C channels: softmax(q k^T / sqrt(C)) v, then to_out + residual"""
         hw = h * w
@@ -232,16 +204,16 @@ class VaeEngine(NetEngine):
         qk = self._linear(plan, prog, g, M, None, 2 * C, w=wqk, bias=bqk)
         # V^T [nb, C, hw_ld] and P [hw, hw_ld]: the kernels never write the pad columns, which the PV product reads,
         # so a recycled block is cleared first
-        vt = self._buf(plan, nb, C, hw_ld)
-        pm = self._buf(plan, hw, hw_ld)
+        vt = plan.pool.buf(nb, C, hw_ld)
+        pm = plan.pool.buf(hw, hw_ld)
         if hw_ld != hw:
             prog.add_memset(vt)
             prog.add_memset(pm)
-        sm = self._buf(plan, hw, hw, dtype=torch.float32)
+        sm = plan.pool.buf(hw, hw, dtype=torch.float32)
         prog.add(ops.gemm_desc(a0=g, w=self.w_linear(name + ".to_v"), out=vt, N_=C, M=M, bias=self.vec(name + ".to_v.bias"),
                                epilogue=N.PP_EPI_TRANSPOSED, t_rows=hw, t_ld=hw_ld))
-        self._free(plan, g)
-        o = self._buf(plan, M, C)
+        plan.pool.free(g)
+        o = plan.pool.buf(M, C)
         scale = 1.0 / math.sqrt(C)
         for b in range(nb):
             rows = qk[b * hw:(b + 1) * hw]
@@ -249,31 +221,21 @@ class VaeEngine(NetEngine):
                                    out_fp32=True))
             prog.add_softmax_rows(sm, pm, hw, hw, hw, hw_ld)
             prog.add(ops.gemm_desc(a0=pm, c0=hw_ld, lda0=hw_ld, w=vt[b], ldb=hw_ld, out=o[b * hw:(b + 1) * hw], N_=C, M=hw))
-        self._free(plan, qk, vt, pm, sm)
+        plan.pool.free(qk, vt, pm, sm)
         out = self._linear(plan, prog, o, M, name + ".to_out.0", C, bias=self.vec(name + ".to_out.0.bias"), res1=x,
                            stats_hw=hw)
-        self._free(plan, o)
+        plan.pool.free(o)
         return out
 
     def _vae_mid(self, plan, prog, name, x, nb, h, w):
         C = x.shape[-1]
-        a = self._vae_resnet(plan, prog, name + ".resnets.0", x, nb, h, w, C)
-        self._free(plan, x)
+        a = self._resnet(plan, prog, name + ".resnets.0", x, None, nb, h, w, C, eps=self.GN_EPS)
+        plan.pool.free(x)
         b = self._vae_attention(plan, prog, name + ".attentions.0", a, nb, h, w)
-        self._free(plan, a)
-        c = self._vae_resnet(plan, prog, name + ".resnets.1", b, nb, h, w, C)
-        self._free(plan, b)
+        plan.pool.free(a)
+        c = self._resnet(plan, prog, name + ".resnets.1", b, None, nb, h, w, C, eps=self.GN_EPS)
+        plan.pool.free(b)
         return c
-
-    def _get_plan(self, key, build):
-        p = self._plans.pop(key, None)
-        if p is None:
-            p = build()
-            p.program.build_graph()
-            while len(self._plans) >= self.MAX_PLANS:
-                self._plans.popitem(last=False)
-        self._plans[key] = p
-        return p
 
     def _check_latent(self, h: int, w: int, what: str):
         if h * w > VAE_MAX_LATENT_PIXELS:
@@ -290,7 +252,7 @@ class VaeEngine(NetEngine):
     # ---- encoder
     def encode_plan(self, nb: int, H: int, W: int) -> Plan:
         self._check_latent(*self._latent_hw(H, W), "encode")
-        return self._get_plan(("enc", nb, H, W), lambda: self._build_encode(nb, H, W))
+        return self._plan(("enc", nb, H, W), lambda: self._build_encode(nb, H, W), graph=True)
 
     def _build_encode(self, nb, H, W, plan: Optional[Plan] = None, x_in: Optional[torch.Tensor] = None,
                       out: Optional[torch.Tensor] = None) -> Plan:
@@ -299,9 +261,7 @@ class VaeEngine(NetEngine):
         cfg = self.cfg
         boc = cfg.block_out_channels
         self._check_latent(*self._latent_hw(H, W), "encode")
-        if plan is None:
-            plan = Plan()
-            plan.program = ops.Program()
+        plan = plan or Plan(Pool(self.device))
         prog = plan.program
         if x_in is None:
             x_in = torch.zeros(nb, H * W, 8, dtype=BF16, device=self.device)
@@ -310,20 +270,21 @@ class VaeEngine(NetEngine):
         cur = self._conv3(plan, prog, x_in, nb, h, w, "encoder.conv_in", boc[0], pad_in=8, stats=True)
         for i, co in enumerate(boc):
             for j in range(cfg.layers_per_block):
-                nxt = self._vae_resnet(plan, prog, f"encoder.down_blocks.{i}.resnets.{j}", cur, nb, h, w, co)
-                self._free(plan, cur)
+                nxt = self._resnet(plan, prog, f"encoder.down_blocks.{i}.resnets.{j}", cur, None, nb, h, w, co,
+                                   eps=self.GN_EPS)
+                plan.pool.free(cur)
                 cur = nxt
             if i != len(boc) - 1:
                 if h < 2 or w < 2:
                     raise ValueError(f"image {H}x{W} is too small for the VAE encoder")
                 nxt = self._conv3(plan, prog, cur, nb, h, w, f"encoder.down_blocks.{i}.downsamplers.0.conv", co,
                                   a_mode=N.PP_A_CONV3X3_S2P0, stats=True)
-                self._free(plan, cur)
+                plan.pool.free(cur)
                 cur = nxt
                 h, w = h // 2, w // 2
         cur = self._vae_mid(plan, prog, "encoder.mid_block", cur, nb, h, w)
         gno = self._gn(plan, prog, cur, None, nb, h * w, "encoder.conv_norm_out", self.GN_EPS, True)
-        self._free(plan, cur)
+        plan.pool.free(cur)
         # conv_out followed by the 1x1 quant_conv: both linear, folded into one conv on the host (fp32)
         lc2 = 2 * cfg.latent_channels
 
@@ -337,7 +298,7 @@ class VaeEngine(NetEngine):
         moments = out if out is not None else torch.empty(nb, h * w, lc2, dtype=torch.float32, device=self.device)
         prog.add(ops.gemm_desc(a0=gno, w=wf, out=moments, N_=lc2, a_mode=N.PP_A_CONV3X3, c0=gno.shape[-1], nb=nb, h=h,
                                w_=w, bias=bf, out_fp32=True))
-        self._free(plan, gno)
+        plan.pool.free(gno)
         if out is None:
             plan.outputs["moments"] = moments
             plan.outputs["hw"] = (h, w)
@@ -346,7 +307,7 @@ class VaeEngine(NetEngine):
     # ---- decoder
     def decode_plan(self, nb: int, h: int, w: int) -> Plan:
         self._check_latent(h, w, "decode")
-        return self._get_plan(("dec", nb, h, w), lambda: self._build_decode(nb, h, w))
+        return self._plan(("dec", nb, h, w), lambda: self._build_decode(nb, h, w), graph=True)
 
     def _build_decode(self, nb, h, w, plan: Optional[Plan] = None, z_in: Optional[torch.Tensor] = None,
                       out: Optional[torch.Tensor] = None) -> Plan:
@@ -356,9 +317,7 @@ class VaeEngine(NetEngine):
         rev = list(reversed(cfg.block_out_channels))
         lc = cfg.latent_channels
         self._check_latent(h, w, "decode")
-        if plan is None:
-            plan = Plan()
-            plan.program = ops.Program()
+        plan = plan or Plan(Pool(self.device))
         prog = plan.program
         if z_in is None:
             z_in = torch.zeros(nb, h * w, 8, dtype=BF16, device=self.device)
@@ -372,24 +331,25 @@ class VaeEngine(NetEngine):
         cur = self._vae_mid(plan, prog, "decoder.mid_block", cur, nb, h, w)
         for i, co in enumerate(rev):
             for j in range(cfg.layers_per_block + 1):
-                nxt = self._vae_resnet(plan, prog, f"decoder.up_blocks.{i}.resnets.{j}", cur, nb, h, w, co)
-                self._free(plan, cur)
+                nxt = self._resnet(plan, prog, f"decoder.up_blocks.{i}.resnets.{j}", cur, None, nb, h, w, co,
+                                   eps=self.GN_EPS)
+                plan.pool.free(cur)
                 cur = nxt
             if i != len(rev) - 1:
-                up = self._buf(plan, nb, 4 * h * w, co)
+                up = plan.pool.buf(nb, 4 * h * w, co)
                 prog.add_upsample_nearest(cur, up, nb, h, w, co, 2 * h, 2 * w)
-                self._free(plan, cur)
+                plan.pool.free(cur)
                 h, w = 2 * h, 2 * w
                 cur = self._conv3(plan, prog, up, nb, h, w, f"decoder.up_blocks.{i}.upsamplers.0.conv", co, stats=True)
-                self._free(plan, up)
+                plan.pool.free(up)
         gno = self._gn(plan, prog, cur, None, nb, h * w, "decoder.conv_norm_out", self.GN_EPS, True)
-        self._free(plan, cur)
+        plan.pool.free(cur)
         # fp32 image, 4 floats per pixel (3 used): the uint8 conversion must not see a bf16-rounded value
         image = out if out is not None else torch.zeros(nb, h * w, 4, dtype=torch.float32, device=self.device)
         prog.add(ops.gemm_desc(a0=gno, w=self.w_conv3("decoder.conv_out"), out=image, N_=cfg.out_channels,
                                a_mode=N.PP_A_CONV3X3, c0=gno.shape[-1], nb=nb, h=h, w_=w,
                                bias=self.vec("decoder.conv_out.bias"), out_fp32=True, ldc=4))
-        self._free(plan, gno)
+        plan.pool.free(gno)
         if out is None:
             plan.outputs["image"] = image
             plan.outputs["hw"] = (h, w)
@@ -401,15 +361,8 @@ class VaeEngine(NetEngine):
     TILE_CHUNK_PIXELS = 4 * 512 * 512
 
     def tiled_plan(self, encode: bool, nb: int, H: int, W: int, geom: VaeTileGeometry, key: tuple) -> Plan:
-        return self._get_plan(("tenc" if encode else "tdec", nb, H, W) + key,
-                              lambda: self._build_tiled(encode, nb, H, W, geom))
-
-    def _restart_gn_arena(self, plan, prog):
-        """the next GroupNorms start over at the head of the current arena, cleared again at this point"""
-        ent = plan.gn_arenas.get(id(prog))
-        if ent is not None and ent[1]:
-            prog.add_memset(ent[0])
-            ent[1] = 0
+        return self._plan(("tenc" if encode else "tdec", nb, H, W) + key,
+                          lambda: self._build_tiled(encode, nb, H, W, geom), graph=True)
 
     def _build_tiled(self, encode: bool, nb: int, H: int, W: int, geom: VaeTileGeometry) -> Plan:
         """ONE program over the whole canvas: per tile shape, gather the tiles of every sample out of the canvas and
@@ -417,13 +370,11 @@ class VaeEngine(NetEngine):
         store; then blend every tile with its upper and left neighbours in diffusers' row-major order, in place;
         then copy each tile's crop into the output. Every chunk records into the plan's one activation pool."""
         cfg = self.cfg
-        plan = Plan()
-        plan.best_fit = True
-        prog = plan.program = ops.Program()
+        plan = Plan(Pool(self.device, best_fit=True))
+        prog = plan.program
         C = 2 * cfg.latent_channels if encode else 4
-        canvas = torch.zeros(nb, H * W, 8, dtype=BF16, device=self.device)
-        out = torch.zeros(nb, geom.out_h * geom.out_w, C, dtype=torch.float32, device=self.device)
-        plan.bytes += canvas.numel() * 2 + out.numel() * 4
+        canvas = plan.pool.tensor(nb, H * W, 8, zero=True)
+        out = plan.pool.tensor(nb, geom.out_h * geom.out_w, C, dtype=torch.float32, zero=True)
         plan.inputs["x" if encode else "z"] = canvas
         build = self._build_encode if encode else self._build_decode
         views: Dict[int, torch.Tensor] = {}  # tile -> fp32 [nb, out_h, out_w, C] in its group's store
@@ -432,19 +383,18 @@ class VaeEngine(NetEngine):
         for (th, tw), idx in sorted(geom.groups().items(), key=lambda g: -g[0][0] * g[0][1]):
             t0 = geom.tiles[idx[0]]
             ohw = t0.out_h * t0.out_w
-            store = torch.zeros(len(idx) * nb, ohw, C, dtype=torch.float32, device=self.device)
-            plan.bytes += store.numel() * 4
+            store = plan.pool.tensor(len(idx) * nb, ohw, C, dtype=torch.float32, zero=True)
             images = [(k, s) for k in idx for s in range(nb)]  # row r of the store holds images[r]
             per = max(1, self.TILE_CHUNK_PIXELS // (th * tw if encode else ohw))
             for r0 in range(0, len(images), per):
                 chunk = images[r0:r0 + per]
-                x_in = self._buf(plan, len(chunk), th * tw, 8)
+                x_in = plan.pool.buf(len(chunk), th * tw, 8)
                 gather = [((s * H * W + geom.tiles[k].y * W + geom.tiles[k].x) * 8, m * th * tw * 8, W * 8, tw * 8,
                            th, tw) for m, (k, s) in enumerate(chunk)]
                 prog.add_window_copy(ops.WindowList(canvas, x_in, 8, gather))
-                self._restart_gn_arena(plan, prog)
+                plan.pool.restart_gn_arena(prog)
                 build(len(chunk), th, tw, plan, x_in, store[r0:r0 + len(chunk)])
-                self._free(plan, x_in)
+                plan.pool.free(x_in)
             crops = []
             for j, k in enumerate(idx):
                 t = geom.tiles[k]

@@ -18,14 +18,13 @@ from __future__ import annotations
 
 from collections import OrderedDict
 from types import SimpleNamespace
-from typing import Dict, List, Optional
+from typing import Optional
 
 import torch
 import torch.nn as nn
 
 from .. import _native as N
-from .. import ops
-from ..engine import BF16, NetEngine, Plan
+from ..engine import BF16, Plan, Pool, Recorder
 
 
 def clip_param_shapes(cfg) -> "OrderedDict[str, tuple]":
@@ -50,32 +49,13 @@ def clip_param_shapes(cfg) -> "OrderedDict[str, tuple]":
     return d
 
 
-class ClipEngine(NetEngine):
+class ClipEngine(Recorder):
     """records the text transformer for a fixed (batch, seq) as one program"""
 
     MAX_PLANS = 4
 
-    def __init__(self, cfg, state_dict: Dict[str, torch.Tensor], device):
-        self.cfg = cfg
-        self.kind = "clip"
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("ClipEngine needs a CUDA device: there is no CPU path")
-        N.lib()
-        self._sd = state_dict
-        self._w: Dict[str, torch.Tensor] = {}
-        self._plans: "OrderedDict[tuple, Plan]" = OrderedDict()
-
     def plan_for(self, nb: int, seq: int, n_ext: int) -> Plan:
-        key = (nb, seq, n_ext)
-        p = self._plans.pop(key, None)
-        if p is None:
-            p = self._build(nb, seq, n_ext)
-            p.program.build_graph()
-            while len(self._plans) >= self.MAX_PLANS:
-                self._plans.popitem(last=False)
-        self._plans[key] = p
-        return p
+        return self._plan((nb, seq, n_ext), lambda: self._build(nb, seq, n_ext), graph=True)
 
     def _build(self, nb, seq, n_ext) -> Plan:
         cfg = self.cfg
@@ -86,43 +66,43 @@ class ClipEngine(NetEngine):
         act = {"quick_gelu": N.PP_ACT_QUICK_GELU}.get(cfg.hidden_act)
         if act is None:
             raise NotImplementedError(f"hidden_act {cfg.hidden_act!r}: the CLIP ViT-L/14 text tower of SD-1.5 uses quick_gelu")
-        plan = Plan()
-        prog = plan.program = ops.Program()
+        plan = Plan(Pool(self.device))
+        prog = plan.program
         idx = torch.zeros(M, dtype=torch.int32, device=self.device)
         ext = torch.zeros(max(n_ext, 1), H, dtype=torch.float32, device=self.device)
         plan.inputs["idx"], plan.inputs["ext"] = idx, ext
         base = self.vec("text_model.embeddings.token_embedding.weight")
         pos = self.vec("text_model.embeddings.position_embedding.weight")
-        x = self._buf(plan, M, H)
+        x = plan.pool.buf(M, H)
         prog.add_embed_gather(idx, base, ext, pos, x, M, base.shape[0], seq, H)
         scale = d ** -0.5
         for i in range(cfg.num_hidden_layers):
             p = f"text_model.encoder.layers.{i}"
-            l1 = self._buf(plan, M, H)
+            l1 = plan.pool.buf(M, H)
             prog.add_layer_norm(x, l1, self.vec(p + ".layer_norm1.weight"), self.vec(p + ".layer_norm1.bias"), M, H, eps)
             wqkv = self._cached("qkv:" + p, lambda p=p: torch.cat(
                 [self._raw(f"{p}.self_attn.{n}.weight") for n in ("q_proj", "k_proj", "v_proj")], 0).to(BF16).contiguous())
             bqkv = self._cached("qkvb:" + p, lambda p=p: torch.cat(
                 [self._raw(f"{p}.self_attn.{n}.bias") for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous())
             qkv = self._linear(plan, prog, l1, M, None, 3 * H, w=wqkv, bias=bqkv)
-            self._free(plan, l1)
-            a = self._buf(plan, M, H)
+            plan.pool.free(l1)
+            a = plan.pool.buf(M, H)
             prog.add_causal_attention_small(qkv, a, nb, seq, heads, d, scale)
-            self._free(plan, qkv)
+            plan.pool.free(qkv)
             x1 = self._linear(plan, prog, a, M, p + ".self_attn.out_proj", H, bias=self.vec(p + ".self_attn.out_proj.bias"),
                               res1=x)
-            self._free(plan, a, x)
-            l2 = self._buf(plan, M, H)
+            plan.pool.free(a, x)
+            l2 = plan.pool.buf(M, H)
             prog.add_layer_norm(x1, l2, self.vec(p + ".layer_norm2.weight"), self.vec(p + ".layer_norm2.bias"), M, H, eps)
             f = self._linear(plan, prog, l2, M, p + ".mlp.fc1", cfg.intermediate_size, bias=self.vec(p + ".mlp.fc1.bias"),
                              act=act)
-            self._free(plan, l2)
+            plan.pool.free(l2)
             x = self._linear(plan, prog, f, M, p + ".mlp.fc2", H, bias=self.vec(p + ".mlp.fc2.bias"), res1=x1)
-            self._free(plan, f, x1)
+            plan.pool.free(f, x1)
         out = torch.empty(M, H, dtype=BF16, device=self.device)
         prog.add_layer_norm(x, out, self.vec("text_model.final_layer_norm.weight"),
                             self.vec("text_model.final_layer_norm.bias"), M, H, eps)
-        self._free(plan, x)
+        plan.pool.free(x)
         plan.outputs["hidden"] = out
         return plan
 

@@ -380,8 +380,7 @@ class BrushNetModel(_HotPathModel):
             shapes_d, shape_m, shapes_u = self.engine()._state_shapes(nb, h, w)
             alphas, pool = self._side_plan_options(guess_mode, len(shapes_d) + 1 + len(shapes_u))
             # one recorded program for every conditioning_scale: the zero-conv epilogues read it from a device scalar
-            plan = self.engine().plan(nb, h, w, encoder_hidden_states.shape[1], brushnet_outputs=True,
-                                      side_alphas=alphas, side_pool=pool)
+            plan = self.engine().plan(nb, h, w, encoder_hidden_states.shape[1], side_alphas=alphas, side_pool=pool)
             plan.scale_dev.fill_(float(conditioning_scale))
             self._load_inputs(plan, sample, timestep, encoder_hidden_states, extra_channels=brushnet_cond)
             plan.program.launch()

@@ -1011,7 +1011,7 @@ class _Census:
 def _capture_all(monkeypatch, census):
     from powerpaint_b200 import ops as o
     from powerpaint_b200.denoise import FusedDenoiser
-    from powerpaint_b200.engine import NetConfig, NetEngine
+    from powerpaint_b200.engine import NetConfig, Recorder
     from powerpaint_b200.models import BrushNetModel, CLIPTextModel, ControlNetModel, UNet2DConditionModel
     from powerpaint_b200.models.autoencoder_kl import AutoencoderKL
 
@@ -1030,7 +1030,7 @@ def _capture_all(monkeypatch, census):
     for sw_name, sw in ENGINE_SWITCHES:
         with monkeypatch.context() as m:
             for attr, val in sw.items():
-                m.setattr(NetEngine, attr, val)
+                m.setattr(Recorder, attr, val)
             for model in (u9, u4, bn, cn):
                 model._engine = None  # repack under the switched options
             for name, mode, B, h, w in DENOISER_SHAPES:
