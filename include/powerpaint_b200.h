@@ -29,6 +29,8 @@
  *   pp_unipc_step     CFG combine + UniPCMultistepScheduler.step (the v2 app's scheduler, app.py:197)
  *   pp_solver_step    CFG combine + DPMSolverMultistepScheduler / EulerDiscreteScheduler /
  *                     EulerAncestralDiscreteScheduler.step (the scheduler a user swaps in, as app.py:197 does)
+ *   pp_plms_step      CFG combine + PNDMScheduler.step with skip_prk_steps (the scheduler stored by the v1
+ *                     checkpoint, app.py:91-93) + 4-channel blend
  *   pp_pool_broadcast spatial mean of a side-net residual, broadcast to full size (global_pool_conditions,
  *                     BrushNet_CA.py:936-943), added onto an optional running Multi-ControlNet sum
  *   pp_upsample_nearest  Upsample2D with an explicit output size (unet_2d_condition.py:1120-1126,1311-1312)
@@ -424,6 +426,39 @@ typedef struct pp_solver_desc {
 } pp_solver_desc;
 pp_status pp_solver_step(const pp_solver_desc* d, pp_stream stream);
 
+/* CFG combine + one step of PNDMScheduler with skip_prk_steps (PLMS: the Heun restart at counter 1, then
+   Adams-Bashforth of order up to 4 on the eps history) + the optional 4-channel blend + next-step input build.
+   Every step is linear in the tensors it touches, so the host folds it into one row of 8 floats (pcoef, computed in
+   float64), with the history already mapped onto physical ring slots:
+     x_next  = r[0] * x + r[1] * cur_sample + r[2] * eps + r[3] * ets[0] + r[4] * ets[1] + r[5] * ets[2]
+     cur_sample <- x                  if r[7] != 0   (the sample a Heun restart starts again from)
+     ets[(int)r[6]] <- eps            if r[6] >= 0   (written after the reads: it may replace the oldest entry)
+     blend (blend_x0 != NULL), as pp_cfg_ddim_desc, with sqrt(alpha_bar) = coef[row][7]
+     latents <- x_next; next_in = bf16(x_next) into channels 0..3 of every copy
+   A term whose weight is exactly 0 is not read. guidance scale = coef[row][5] of the shared 8-float table.
+   latents, cur_sample and every ring slot are fp32 NHWC [batch, hw, 4]; ets holds the 3 slots back to back
+   ([3, batch, hw, 4]); all of them 16-byte aligned. */
+typedef struct pp_plms_desc {
+    const void* eps;     /* as pp_unipc_desc: [n_copies*batch, hw, eps_ld] fp32 or bf16, unconditional half first */
+    int32_t eps_fp32;
+    int32_t eps_ld;
+    float* latents;
+    float* cur_sample;
+    float* ets;
+    const float* coef;   /* [n_steps, 8], column 5 = guidance scale, column 7 = the blend's sqrt(alpha_bar) */
+    const float* pcoef;  /* [n_steps, 8] */
+    int32_t* step_idx;
+    int32_t advance_step;
+    int32_t do_cfg;
+    int32_t batch, hw;
+    void* next_in;       /* bf16 NHWC [n_copies*batch, hw, next_c]: channels 0..3 refreshed */
+    int32_t next_c, n_copies;
+    const float* blend_x0;     /* as pp_cfg_ddim_desc: [hw, 4] fp32, all three NULL or all set */
+    const float* blend_mask;   /* [hw] fp32 */
+    const float* blend_noise;  /* [batch, hw, 4] fp32 */
+} pp_plms_desc;
+pp_status pp_plms_step(const pp_plms_desc* d, pp_stream stream);
+
 /* ------------------------------------------------------------------ side-net global pooling */
 /* Global pooling of a side net's residual (`global_pool_conditions`: BrushNet_CA.py:936-943, diffusers
    ControlNetModel): for every sample s, pixel p and channel c of the bf16 NHWC [batch, hw, channels] buffers
@@ -460,6 +495,7 @@ pp_status pp_program_add_time_embed(pp_program* p, const float* timesteps,
 pp_status pp_program_add_cfg_ddim(pp_program* p, const pp_cfg_ddim_desc* d);
 pp_status pp_program_add_unipc(pp_program* p, const pp_unipc_desc* d);
 pp_status pp_program_add_solver_step(pp_program* p, const pp_solver_desc* d);
+pp_status pp_program_add_plms_step(pp_program* p, const pp_plms_desc* d);
 pp_status pp_program_add_memset(pp_program* p, void* ptr, int64_t bytes);
 pp_status pp_program_add_embed_gather(pp_program* p, const int32_t* idx, const float* base, const float* ext,
                                       const float* pos, void* out, int32_t rows, int32_t vocab, int32_t seq, int32_t dim);

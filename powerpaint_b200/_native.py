@@ -112,6 +112,17 @@ class SolverDesc(C.Structure):
     ]
 
 
+class PlmsDesc(C.Structure):
+    _fields_ = [
+        ("eps", vp), ("eps_fp32", i32), ("eps_ld", i32),
+        ("latents", vp), ("cur_sample", vp), ("ets", vp),
+        ("coef", vp), ("pcoef", vp), ("step_idx", vp), ("advance_step", i32), ("do_cfg", i32),
+        ("batch", i32), ("hw", i32),
+        ("next_in", vp), ("next_c", i32), ("n_copies", i32),
+        ("blend_x0", vp), ("blend_mask", vp), ("blend_noise", vp),
+    ]
+
+
 class Window(C.Structure):
     _fields_ = [("src_off", i64), ("dst_off", i64), ("src_row", i64), ("dst_row", i64), ("rows", i32), ("cols", i32)]
 
@@ -157,6 +168,8 @@ _SIGNATURES = {
     "pp_program_add_unipc": (C.c_int, [vp, C.POINTER(UniPCDesc)]),
     "pp_solver_step": (C.c_int, [C.POINTER(SolverDesc), vp]),
     "pp_program_add_solver_step": (C.c_int, [vp, C.POINTER(SolverDesc)]),
+    "pp_plms_step": (C.c_int, [C.POINTER(PlmsDesc), vp]),
+    "pp_program_add_plms_step": (C.c_int, [vp, C.POINTER(PlmsDesc)]),
     "pp_softmax_rows": (C.c_int, [vp, vp, i64, i32, i64, i64, vp]),
     "pp_embed_gather": (C.c_int, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "pp_causal_attention_small": (C.c_int, [vp, vp, i32, i32, i32, i32, f32, vp]),

@@ -316,6 +316,128 @@ int solver_launch(const pp_solver_desc& d, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------
+// Fused CFG + one step of PNDMScheduler with skip_prk_steps (PLMS) + 4-channel blend + next-input refresh.
+// Every PLMS step is linear in (x, cur_sample, eps, the earlier eps in the history ring), so the host folds it into
+// one 8-float row (include/powerpaint_b200.h, pp_plms_desc) that already names the physical ring slots: the kernel
+// never shifts history. A weight of exactly zero skips its load (uniform per launch), so a ring slot or cur_sample
+// that has never been written is never read. One thread per pixel, 16-byte accesses. Algorithmic bytes per pixel
+// (CFG, fp32 eps, 4-entry AB step): eps 32 + latents 16 + 16 + ring 3 x 16 + 16 + next input 2 x 8 = 144 B; the
+// Heun restart (counter 1) reads cur_sample and one slot instead.
+// ------------------------------------------------------------------------------------
+__global__ void plms_step_kernel(pp_plms_desc d) {
+    pdl_wait();
+    pdl_launch_dependents();
+    const int64_t total = (int64_t)d.batch * d.hw;
+    const int step = d.step_idx ? *d.step_idx : 0;
+    const float* cf = d.coef + (int64_t)step * 8;
+    const float gscale = cf[5];
+    const float* r = d.pcoef + (int64_t)step * 8;
+    const float wx = r[0], wc = r[1], we = r[2];
+    const float wh[3] = {r[3], r[4], r[5]};
+    const int slot = (int)r[6];  // ring slot the new eps goes to, -1 = none
+    const bool save_cur = r[7] != 0.f;
+    const int64_t slot_stride = total * 4;
+    const bool eps_vec = d.eps_fp32 && d.eps_ld == 4;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+         i += (int64_t)gridDim.x * blockDim.x) {
+        float eu[4], ec[4];
+        if (eps_vec) {
+            const float4* e = reinterpret_cast<const float4*>(d.eps);
+            const float4 a = __ldg(e + i), c = __ldg(e + i + (d.do_cfg ? total : 0));
+            eu[0] = a.x; eu[1] = a.y; eu[2] = a.z; eu[3] = a.w;
+            ec[0] = c.x; ec[1] = c.y; ec[2] = c.z; ec[3] = c.w;
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int64_t iu = i * d.eps_ld + j, ic = (i + (d.do_cfg ? total : 0)) * d.eps_ld + j;
+                eu[j] = d.eps_fp32 ? reinterpret_cast<const float*>(d.eps)[iu]
+                                   : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(d.eps)[iu]);
+                ec[j] = d.eps_fp32 ? reinterpret_cast<const float*>(d.eps)[ic]
+                                   : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(d.eps)[ic]);
+            }
+        }
+        const float4 x4 = *reinterpret_cast<const float4*>(d.latents + i * 4);
+        const float x[4] = {x4.x, x4.y, x4.z, x4.w};
+        float eps[4], xn[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            eps[j] = d.do_cfg ? eu[j] + gscale * (ec[j] - eu[j]) : eu[j];
+            xn[j] = we * eps[j];
+        }
+        if (wx != 0.f) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) xn[j] += wx * x[j];
+        }
+        if (wc != 0.f) {
+            const float4 c4 = *reinterpret_cast<const float4*>(d.cur_sample + i * 4);
+            xn[0] += wc * c4.x; xn[1] += wc * c4.y; xn[2] += wc * c4.z; xn[3] += wc * c4.w;
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            if (wh[k] != 0.f) {
+                const float4 h4 = *reinterpret_cast<const float4*>(d.ets + k * slot_stride + i * 4);
+                xn[0] += wh[k] * h4.x; xn[1] += wh[k] * h4.y; xn[2] += wh[k] * h4.z; xn[3] += wh[k] * h4.w;
+            }
+        }
+        // history writes after every read of this pixel: the new eps may replace the oldest entry this step read
+        if (save_cur) *reinterpret_cast<float4*>(d.cur_sample + i * 4) = x4;
+        if (slot >= 0)
+            *reinterpret_cast<float4*>(d.ets + slot * slot_stride + i * 4) = make_float4(eps[0], eps[1], eps[2], eps[3]);
+        if (d.blend_x0) {
+            // 4-channel UNet: keep the known region on the noised original (pipeline_PowerPaint.py:1025-1035)
+            const float a = cf[7], s1a = sqrtf(fmaxf(1.f - a * a, 0.f));
+            const int64_t pix = i % d.hw;
+            const float m = __ldg(d.blend_mask + pix);
+            const float4 o4 = __ldg(reinterpret_cast<const float4*>(d.blend_x0) + pix);
+            const float4 n4 = __ldg(reinterpret_cast<const float4*>(d.blend_noise) + i);
+            const float o[4] = {o4.x, o4.y, o4.z, o4.w}, nn[4] = {n4.x, n4.y, n4.z, n4.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) xn[j] = (1.f - m) * (a * o[j] + s1a * nn[j]) + m * xn[j];
+        }
+        *reinterpret_cast<float4*>(d.latents + i * 4) = make_float4(xn[0], xn[1], xn[2], xn[3]);
+        if (d.next_in) {
+            __nv_bfloat16* ni = reinterpret_cast<__nv_bfloat16*>(d.next_in);
+            const uint2 v = make_uint2(pack_bf16x2(xn[0], xn[1]), pack_bf16x2(xn[2], xn[3]));
+            for (int cpy = 0; cpy < d.n_copies; ++cpy)
+                *reinterpret_cast<uint2*>(ni + ((int64_t)cpy * total + i) * d.next_c) = v;
+        }
+    }
+}
+
+int plms_validate(const pp_plms_desc& d) {
+    PP_REQUIRE(d.eps && d.latents && d.cur_sample && d.ets && d.coef && d.pcoef, "plms: null pointer");
+    PP_REQUIRE(d.batch > 0 && d.hw > 0 && d.eps_ld >= 4, "plms: invalid shape");
+    PP_REQUIRE(!d.advance_step || d.step_idx, "plms: advance_step needs step_idx");
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(d.latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.cur_sample) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(d.ets) & 15) == 0,
+               "plms: latents / cur_sample / ets need 16-byte alignment");
+    PP_REQUIRE(!(d.eps_fp32 && d.eps_ld == 4) || (reinterpret_cast<uintptr_t>(d.eps) & 15) == 0,
+               "plms: fp32 eps with eps_ld 4 needs 16-byte alignment");
+    PP_REQUIRE((d.blend_x0 == nullptr) == (d.blend_mask == nullptr) && (d.blend_x0 == nullptr) == (d.blend_noise == nullptr),
+               "plms: blend_x0 / blend_mask / blend_noise go together");
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(d.blend_x0) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.blend_noise) & 15) == 0,
+               "plms: blend_x0 / blend_noise need 16-byte alignment");
+    if (d.next_in)
+        PP_REQUIRE(d.next_c >= 4 && d.next_c % 4 == 0 && d.n_copies >= 1 && (reinterpret_cast<uintptr_t>(d.next_in) & 7) == 0,
+                   "plms: next_in needs next_c %% 4 == 0, n_copies >= 1 and 8-byte alignment");
+    return PP_OK;
+}
+
+int plms_launch(const pp_plms_desc& d, cudaStream_t s) {
+    int rc = plms_validate(d);
+    if (rc) return rc;
+    const int64_t total = (int64_t)d.batch * d.hw;
+    const int blocks = (int)std::min<int64_t>((total + 127) / 128, 132 * 8);
+    PP_CUDA_CHECK(launch(plms_step_kernel, blocks, 128, 0, s, d));
+    PP_CUDA_CHECK(cudaGetLastError());
+    if (d.advance_step) {
+        PP_CUDA_CHECK(launch(cfg_ddim_advance_kernel, 1, 1, 0, s, d.step_idx));
+        PP_CUDA_CHECK(cudaGetLastError());
+    }
+    return PP_OK;
+}
+
+// ------------------------------------------------------------------------------------
 // Timesteps(dim, flip_sin_to_cos=True, downscale_freq_shift=0)
 // (powerpaint/models/unet_2d_condition.py:914-938): emb = [cos(t f_i), sin(t f_i)],
 // f_i = exp(-ln(10000) i / half).
@@ -508,6 +630,10 @@ pp_status pp_unipc_step(const pp_unipc_desc* d, pp_stream s) {
 pp_status pp_solver_step(const pp_solver_desc* d, pp_stream s) {
     if (!d) { pp::set_last_error("pp_solver_step: null descriptor"); return pp::PP_ERR_INVALID; }
     return pp::solver_launch(*d, reinterpret_cast<cudaStream_t>(s));
+}
+pp_status pp_plms_step(const pp_plms_desc* d, pp_stream s) {
+    if (!d) { pp::set_last_error("pp_plms_step: null descriptor"); return pp::PP_ERR_INVALID; }
+    return pp::plms_launch(*d, reinterpret_cast<cudaStream_t>(s));
 }
 pp_status pp_cfg_ddim_step(const pp_cfg_ddim_desc* d, pp_stream s) {
     if (!d) { pp::set_last_error("pp_cfg_ddim_step: null descriptor"); return pp::PP_ERR_INVALID; }

@@ -136,6 +136,8 @@ int unipc_validate(const pp_unipc_desc& d);
 int unipc_launch(const pp_unipc_desc& d, cudaStream_t s);
 int solver_validate(const pp_solver_desc& d);
 int solver_launch(const pp_solver_desc& d, cudaStream_t s);
+int plms_validate(const pp_plms_desc& d);
+int plms_launch(const pp_plms_desc& d, cudaStream_t s);
 int pool_broadcast_validate(const pp_pool_broadcast_desc& d);
 int pool_broadcast_launch(const pp_pool_broadcast_desc& d, cudaStream_t s);
 

@@ -17,7 +17,7 @@ namespace pp {
 
 enum OpKind {
     OP_GEMM, OP_ATTN, OP_GN, OP_LN, OP_UPSAMPLE, OP_ADD, OP_TIME_EMBED, OP_CFG_DDIM, OP_MEMSET, OP_SOFTMAX, OP_UNIPC, OP_EMBED, OP_CAUSAL_ATTN,
-    OP_WINDOW_COPY, OP_TILE_BLEND, OP_SOLVER, OP_POOL_BROADCAST
+    OP_WINDOW_COPY, OP_TILE_BLEND, OP_SOLVER, OP_POOL_BROADCAST, OP_PLMS
 };
 
 struct LnArgs { const void* x; void* y; const float* gamma; const float* beta; int rows, c; float eps; };
@@ -50,6 +50,7 @@ struct Op {
         pp_tile_blend_desc tb;
         pp_solver_desc solver;
         pp_pool_broadcast_desc pool;
+        pp_plms_desc plms;
     };
     Op() { memset(this, 0, sizeof(*this)); }
 };
@@ -86,6 +87,7 @@ static int run_op(const Op& op, cudaStream_t s) {
         case OP_TILE_BLEND: return tile_blend_launch(op.tb, s);
         case OP_SOLVER: return solver_launch(op.solver, s);
         case OP_POOL_BROADCAST: return pool_broadcast_launch(op.pool, s);
+        case OP_PLMS: return plms_launch(op.plms, s);
     }
     set_last_error("program: unknown op kind %d", (int)op.kind);
     return PP_ERR_INVALID;
@@ -97,6 +99,7 @@ static int launches_of(const Op& op) {
         case OP_CFG_DDIM: return op.ddim.advance_step ? 2 : 1;
         case OP_UNIPC: return op.unipc.advance_step ? 2 : 1;
         case OP_SOLVER: return op.solver.advance_step ? 2 : 1;
+        case OP_PLMS: return op.plms.advance_step ? 2 : 1;
         case OP_MEMSET: return 0;
         default: return 1;
     }
@@ -251,6 +254,18 @@ pp_status pp_program_add_solver_step(pp_program* p, const pp_solver_desc* d) {
     pp::Op op;
     op.kind = pp::OP_SOLVER;
     op.solver = *d;
+    p->ops.push_back(op);
+    return pp::PP_OK;
+}
+
+pp_status pp_program_add_plms_step(pp_program* p, const pp_plms_desc* d) {
+    PP_PROG_CHECK(p);
+    if (!d) { pp::set_last_error("pp_program_add_plms_step: null descriptor"); return pp::PP_ERR_INVALID; }
+    int rc = pp::plms_validate(*d);
+    if (rc) return rc;
+    pp::Op op;
+    op.kind = pp::OP_PLMS;
+    op.plms = *d;
     p->ops.push_back(op);
     return pp::PP_OK;
 }

@@ -47,6 +47,7 @@ import torch
 
 from . import ops
 from .engine import NetEngine, Pool, SideOutputs, guess_mode_alphas, lru_get
+from .schedulers import PLMS_RING
 
 MAX_STEPS = 1000
 X_IN_C = 16
@@ -155,6 +156,18 @@ class FusedDenoiser:
                 st["blend_x0"] = torch.zeros(h * w, 4, dtype=torch.float32, device=dev)
                 st["blend_mask"] = torch.zeros(h * w, dtype=torch.float32, device=dev)
                 st["blend_noise"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
+        if sched == "plms":
+            # PNDM / PLMS (the v1 checkpoint's scheduler): the first step's sample and a ring of 3 earlier eps
+            st["cur_sample"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
+            st["ets"] = torch.zeros(PLMS_RING, B, h * w, 4, dtype=torch.float32, device=dev)
+            st["pcoef"] = torch.zeros(MAX_STEPS, 8, dtype=torch.float32, device=dev)
+            prog.add(ops.plms_desc(eps=uplan.outputs["eps"], eps_fp32=True, eps_ld=4, latents=st["latents"],
+                                   cur_sample=st["cur_sample"], ets=st["ets"], coef=coef, pcoef=st["pcoef"],
+                                   step_idx=step_idx, advance_step=True, do_cfg=do_cfg, batch=B, hw=h * w,
+                                   next_in=x_in, next_c=X_IN_C, n_copies=2 if do_cfg else 1,
+                                   blend_x0=st.get("blend_x0"), blend_mask=st.get("blend_mask"),
+                                   blend_noise=st.get("blend_noise")))
+        elif sched == "ddim":
             prog.add(ops.cfg_ddim_desc(eps=uplan.outputs["eps"], eps_fp32=True, eps_ld=4, latents=st["latents"],
                                        coef=coef, step_idx=step_idx, advance_step=True,
                                        noise=st["noise"] if with_noise else None, guidance_scale=0.0,
@@ -185,7 +198,7 @@ class FusedDenoiser:
             side_prompt_embeds: Optional[torch.Tensor] = None, control_image: Optional[torch.Tensor] = None,
             side_scale=1.0, side_keep=None,
             noise_fn: Optional[Callable[[int], torch.Tensor]] = None, ucoef: Optional[torch.Tensor] = None,
-            scoef: Optional[torch.Tensor] = None, blend: Optional[dict] = None,
+            scoef: Optional[torch.Tensor] = None, pcoef: Optional[torch.Tensor] = None, blend: Optional[dict] = None,
             callback: Optional[Callable[[int, int, torch.Tensor], Optional[torch.Tensor]]] = None,
             use_graph: bool = True, guess_mode: bool = False) -> torch.Tensor:
         """latents [B,4,h,w]; prompt_embeds [nb,77,768] for the UNet (negative half first when CFG);
@@ -196,7 +209,10 @@ class FusedDenoiser:
         the eta > 0 variance noise of step i; `ucoef` [n,12] (`UniPCMultistepScheduler.unipc_coefficients`) selects
         the UniPC step kernel instead of DDIM; `scoef` [n,8] (`solver_coefficients` of DPMSolverMultistepScheduler,
         EulerDiscreteScheduler, EulerAncestralDiscreteScheduler) selects `pp_solver_step`, with `noise_fn(i)` the
-        noise of a stochastic step and column 7 of row 0 the input scale of the first step; `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
+        noise of a stochastic step and column 7 of row 0 the input scale of the first step; `pcoef` [n,8]
+        (`PNDMScheduler.plms_coefficients`) selects `pp_plms_step`, whose rows carry the whole PLMS state machine
+        (a callback's replacement latents after step 0 only feed step 1's net input: that step restarts from the
+        sample step 0 started at, as in diffusers); `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
         sqrt_alpha [n]) is the 4-channel-UNet blend (ref pipeline_PowerPaint.py:1025-1035).
         `callback(i, t, latents_nchw)` may return replacement
         latents. Returns the final latents [B,4,h,w] fp32.
@@ -230,9 +246,12 @@ class FusedDenoiser:
         cur = torch.cuda.current_stream(dev)
         self._stream.wait_stream(cur)
         with torch.cuda.device(dev), torch.cuda.stream(self._stream):
-            if ucoef is not None and scoef is not None:
-                raise ValueError("ucoef and scoef select different step kernels: pass one")
-            sched = "unipc" if ucoef is not None else "solver" if scoef is not None else "ddim"
+            if sum(c is not None for c in (ucoef, scoef, pcoef)) > 1:
+                raise ValueError("ucoef, scoef and pcoef select different step kernels: pass one")
+            sched = "unipc" if ucoef is not None else "solver" if scoef is not None else \
+                "plms" if pcoef is not None else "ddim"
+            if sched == "plms" and noise_fn is not None:
+                raise NotImplementedError("PNDM has no stochastic step: noise_fn is DDIM / solver-only")
             if sched == "unipc" and (noise_fn is not None or blend is not None):
                 raise NotImplementedError("eta / the 4-channel blend are DDIM-only on the fused path")
             if sched == "solver" and blend is not None:
@@ -245,6 +264,12 @@ class FusedDenoiser:
                 st["ucoef"][:n_steps].copy_(ucoef.to(dev, torch.float32))
                 for k in ("last_sample", "m1", "m2"):
                     st[k].zero_()
+            if sched == "plms":
+                if len(pcoef) != n_steps:
+                    raise ValueError("pcoef needs one row per step")
+                st["pcoef"][:n_steps].copy_(pcoef.to(dev, torch.float32))
+                st["cur_sample"].zero_()
+                st["ets"].zero_()
             in_scale = lambda i: 1.0  # noqa: E731  (scale_model_input of step i)
             if sched == "solver":
                 if len(scoef) != n_steps:

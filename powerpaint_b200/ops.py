@@ -295,6 +295,23 @@ def solver_desc(*, eps, eps_fp32, eps_ld, latents, m1, coef, scoef, step_idx, ad
     return Desc("solver", d, (eps, latents, m1, noise, coef, scoef, step_idx, next_in))
 
 
+def plms_desc(*, eps, eps_fp32, eps_ld, latents, cur_sample, ets, coef, pcoef, step_idx, advance_step, do_cfg,
+              batch, hw, next_in=None, next_c=0, n_copies=0, blend_x0=None, blend_mask=None,
+              blend_noise=None) -> Desc:
+    """pp_plms_step (include/powerpaint_b200.h): CFG + one folded PNDM (PLMS) step + optional 4-channel blend;
+    `ets` is the [3, batch, hw, 4] fp32 history ring"""
+    d = N.PlmsDesc()
+    d.eps, d.eps_fp32, d.eps_ld = N.ptr(eps), 1 if eps_fp32 else 0, eps_ld
+    d.latents, d.cur_sample, d.ets = N.ptr(latents), N.ptr(cur_sample), N.ptr(ets)
+    d.coef, d.pcoef, d.step_idx = N.ptr(coef), N.ptr(pcoef), N.ptr(step_idx)
+    d.advance_step, d.do_cfg = 1 if advance_step else 0, 1 if do_cfg else 0
+    d.batch, d.hw = batch, hw
+    d.next_in, d.next_c, d.n_copies = N.ptr(next_in), next_c, n_copies
+    d.blend_x0, d.blend_mask, d.blend_noise = N.ptr(blend_x0), N.ptr(blend_mask), N.ptr(blend_noise)
+    return Desc("plms", d, (eps, latents, cur_sample, ets, coef, pcoef, step_idx, next_in, blend_x0, blend_mask,
+                            blend_noise))
+
+
 def _tile_view(t: torch.Tensor, name: str):
     """fp32 [batch, h, w, channels] with every sample contiguous (samples may sit any stride apart)"""
     if t.dtype != torch.float32 or t.dim() != 4 or not t.is_cuda:
@@ -394,6 +411,8 @@ def run(desc: Desc) -> None:
         N.check(L.pp_unipc_step(C.byref(desc.c), s), "pp_unipc_step")
     elif desc.kind == "solver":
         N.check(L.pp_solver_step(C.byref(desc.c), s), "pp_solver_step")
+    elif desc.kind == "plms":
+        N.check(L.pp_plms_step(C.byref(desc.c), s), "pp_plms_step")
     elif desc.kind == "tile_blend":
         N.check(L.pp_tile_blend(C.byref(desc.c), s), "pp_tile_blend")
     elif desc.kind == "pool_broadcast":
@@ -527,7 +546,8 @@ class Program:
         fn = {"gemm": L.pp_program_add_gemm, "attn": L.pp_program_add_attention,
               "gn": L.pp_program_add_group_norm, "cfg_ddim": L.pp_program_add_cfg_ddim,
               "unipc": L.pp_program_add_unipc, "tile_blend": L.pp_program_add_tile_blend,
-              "solver": L.pp_program_add_solver_step, "pool_broadcast": L.pp_program_add_pool_broadcast}[desc.kind]
+              "solver": L.pp_program_add_solver_step, "pool_broadcast": L.pp_program_add_pool_broadcast,
+              "plms": L.pp_program_add_plms_step}[desc.kind]
         N.check(fn(self._h, C.byref(desc.c)), f"pp_program_add_{desc.kind}")
         self._keep.append(desc.keep)
         self.labels.append(desc.kind)

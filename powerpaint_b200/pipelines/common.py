@@ -60,6 +60,13 @@ def solver_loop_inputs(scheduler, timesteps, shape, generator, device):
     return scoef, (draw if scheduler.stochastic else None), finish
 
 
+def callback_fires(i: int, n_timesteps: int, num_warmup_steps: int, order: int) -> bool:
+    """whether the reference loops report step `i` to the legacy `callback` (ref:…pipeline_PowerPaint.py:1038):
+    the last step, and every `order`-th step after `num_warmup_steps = len(timesteps) - num_inference_steps * order`
+    (PNDM: 1, so its first step is not reported; every other scheduler here: 0)"""
+    return i == n_timesteps - 1 or ((i + 1) > num_warmup_steps and (i + 1) % order == 0)
+
+
 def prepare_mask_and_masked_image(image, mask, height, width, return_image: bool = False):
     """(mask [B,1,H,W] in {0,1}, masked_image [B,3,H,W] in [-1,1]) from PIL / numpy / tensor inputs;
     same accepted types, range checks and exceptions as the reference (:39-153)."""

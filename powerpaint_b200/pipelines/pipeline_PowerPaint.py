@@ -19,8 +19,8 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, decode_latents, encode_text, prepare_mask_and_masked_image,
-                     randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
+from .common import (StableDiffusionPipelineOutput, callback_fires, decode_latents, encode_text,
+                     prepare_mask_and_masked_image, randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
 
 
 class StableDiffusionInpaintPipeline:
@@ -130,8 +130,12 @@ class StableDiffusionInpaintPipeline:
             if stored not in (None, "DDIMScheduler"):
                 import warnings
 
+                hint = (" (PLMS runs on the fused loop when chosen explicitly: pipe.scheduler = "
+                        "PNDMScheduler.from_pretrained(checkpoint, subfolder='scheduler'))" if stored == "PNDMScheduler"
+                        else "")
                 warnings.warn(f"powerpaint_b200: the stored scheduler {stored} is replaced by DDIMScheduler built from "
-                              "the same noise schedule (the fused step kernels implement DDIM, UniPC, DPM-Solver++ and Euler)", stacklevel=3)
+                              "the same noise schedule (the fused step kernels implement DDIM, UniPC, DPM-Solver++, "
+                              f"Euler and PNDM){hint}", stacklevel=3)
             return DDIMScheduler.from_config(cfg)
         raise ValueError(f"unknown pipeline component {name!r} ({entry})")
 
@@ -431,11 +435,13 @@ class StableDiffusionInpaintPipeline:
         if not hasattr(self.scheduler, "step_coefficients"):
             raise TypeError("the fused loop needs powerpaint_b200.schedulers.DDIMScheduler (step_coefficients)")
         coef = self.scheduler.step_coefficients(timesteps, eta=extra_step_kwargs.get("eta", 0.0))
-        ucoef = scoef = None
+        ucoef = scoef = pcoef = None
         finish = None
         kind = getattr(self.scheduler, "kind", "ddim")
         if kind == "unipc":
             ucoef = self.scheduler.unipc_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
+        if kind == "plms":
+            pcoef = self.scheduler.plms_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
         blend = None
         if num_channels_unet == 4:
             # 4-channel UNet (:1025-1035): after every step the known region is reset to the original latents noised
@@ -454,17 +460,20 @@ class StableDiffusionInpaintPipeline:
             scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
+            n_ts = len(timesteps)
+            warmup = n_ts - num_inference_steps * self.scheduler.order  # PNDM: 1, its first step is not reported
+
             def cb(i, t, lat):
-                if i % callback_steps == 0:
+                if callback_fires(i, n_ts, warmup, self.scheduler.order) and i % callback_steps == 0:
                     callback(i, t, lat)
                 return None
-        # `scoef` is passed only when a solver scheduler is set: a denoiser whose `run` predates the solver kind
-        # (no `scoef` parameter) keeps serving DDIM and UniPC unchanged
+        # `scoef` / `pcoef` are passed only when such a scheduler is set: a denoiser whose `run` predates those kinds
+        # keeps serving DDIM and UniPC unchanged
+        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, timesteps=timesteps, coef=coef,
                                       guidance_scale=guidance_scale,
                                       extra=torch.cat([mask, masked_image_latents], dim=1) if num_channels_unet == 9
-                                      else None, noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb,
-                                      **({} if scoef is None else dict(scoef=scoef)))
+                                      else None, noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb, **opt)
         if finish is not None:
             finish()
         image = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)

@@ -20,8 +20,9 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import BrushNetModel, UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, check_control_guidance, check_image, check_prompt_arguments,
-                     decode_latents, encode_text, preprocess_image, randn_tensor, solver_loop_inputs)
+from .common import (StableDiffusionPipelineOutput, callback_fires, check_control_guidance, check_image,
+                     check_prompt_arguments, decode_latents, encode_text, preprocess_image, randn_tensor,
+                     solver_loop_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
 
@@ -289,6 +290,7 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         # the v2 app runs UniPC (app.py:197): its folded per-step scalars select the UniPC step kernel
         kind = getattr(self.scheduler, "kind", "ddim")
         ucoef = self.scheduler.unipc_coefficients() if kind == "unipc" else None
+        pcoef = self.scheduler.plms_coefficients() if kind == "plms" else None
         scoef = finish = None
         noise_fn = None
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
@@ -299,6 +301,8 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         cb = None
         if callback_on_step_end is not None or callback is not None:
             pipe = self
+            order = self.scheduler.order
+            warmup = len(ts) - num_inference_steps * order  # PNDM: 1, its first step is not reported to `callback`
 
             def cb(i, t, lat):
                 new = None
@@ -315,12 +319,13 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
                                 "prompt are projected once per call, replacing them mid-loop is not supported")
                     new = outs.pop("latents", lat)
                     lat = new
-                if callback is not None and i % (callback_steps or 1) == 0:
+                fires = callback_fires(i, len(ts), warmup, order) and i % (callback_steps or 1) == 0
+                if callback is not None and fires:
                     callback(i, t, lat)
                 return new
         # `scoef` / `guess_mode` are passed only when set: a denoiser whose `run` predates them keeps serving DDIM
         # and UniPC unchanged
-        opt = {} if scoef is None else dict(scoef=scoef)
+        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
         if guess_mode:
             opt["guess_mode"] = True
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds,

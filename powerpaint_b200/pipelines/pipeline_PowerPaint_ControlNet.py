@@ -19,9 +19,9 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import ControlNetModel, MultiControlNetModel, UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, check_control_guidance, check_image, check_prompt_arguments,
-                     decode_latents, prepare_mask_and_masked_image, preprocess_image, randn_tensor,
-                     solver_loop_inputs, uint8_device_inputs)
+from .common import (StableDiffusionPipelineOutput, callback_fires, check_control_guidance, check_image,
+                     check_prompt_arguments, decode_latents, prepare_mask_and_masked_image, preprocess_image,
+                     randn_tensor, solver_loop_inputs, uint8_device_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
 logger = logging.getLogger(__name__)
@@ -199,11 +199,13 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         # `controlnet_keep` (ref:pipeline_PowerPaint_ControlNet.py:1652-1658): the per-step scale
         # conditioning_scale * keep[i] sits in the device coefficient table the recorded program indexes
         coef = self.scheduler.step_coefficients(timesteps, eta=extra_step_kwargs.get("eta", 0.0))
-        ucoef = scoef = None
+        ucoef = scoef = pcoef = None
         finish = None
         kind = getattr(self.scheduler, "kind", "ddim")
         if kind == "unipc":
             ucoef = self.scheduler.unipc_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
+        if kind == "plms":
+            pcoef = self.scheduler.plms_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
         noise_fn = None
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
             shape = latents.shape
@@ -214,8 +216,11 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
+            n_ts = len(timesteps)
+            warmup = n_ts - num_inference_steps * self.scheduler.order  # PNDM: 1, its first step is not reported
+
             def cb(i, t, lat):
-                if i % callback_steps == 0:
+                if callback_fires(i, n_ts, warmup, self.scheduler.order) and i % callback_steps == 0:
                     callback(i, t, lat)
                 return None
         if multi:
@@ -232,6 +237,8 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             side["guess_mode"] = True
         if scoef is not None:
             side["scoef"] = scoef
+        if pcoef is not None:
+            side["pcoef"] = pcoef
         latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds,
                                       timesteps=timesteps, coef=coef, guidance_scale=guidance_scale,
                                       extra=torch.cat([mask, masked_image_latents], dim=1),

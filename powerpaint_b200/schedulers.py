@@ -726,3 +726,163 @@ class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
         r[2] = s_down / s
         r[3] = 1.0 - s_down / s
         r[5] = s_up
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# PNDM with skip_prk_steps (PLMS): one folded row per step for `pp_plms_step`
+# ---------------------------------------------------------------------------------------------------------------------
+PLMS_RING = 3  # physical eps history slots: a 4-entry Adams-Bashforth step reads the 3 previous entries
+
+
+class _PlmsFold:
+    """The state machine of diffusers' `PNDMScheduler.step_plms`, run on symbols instead of tensors: `row(t)` returns
+    the step at timestep `t` as one row of 8 floats for `pp_plms_step`
+
+        x_next = r0 x + r1 cur_sample + r2 eps + r3 ets[0] + r4 ets[1] + r5 ets[2]
+        ets[r6] <- eps (r6 >= 0);  cur_sample <- x (r7 != 0)
+
+    Appended history entries go to slots 0, 1, 2, 0, ... so a new entry replaces the oldest of the three it can
+    see, which this step reads before the kernel writes it. `alpha(t)` is alpha_bar as diffusers indexes it."""
+
+    AB = {1: (1.0,), 2: (3 / 2, -1 / 2), 3: (23 / 12, -16 / 12, 5 / 12), 4: (55 / 24, -59 / 24, 37 / 24, -9 / 24)}
+
+    def __init__(self, ratio: int, alpha, final_alpha: float):
+        self.ratio, self.alpha, self.final_alpha = ratio, alpha, final_alpha
+        self.counter = 0
+        self.appended = 0
+        self.hist: List[int] = []  # slots of the remembered eps, oldest first (at most 3)
+
+    def row(self, timestep) -> List[float]:
+        t = int(timestep)
+        prev = t - self.ratio
+        r = [0.0] * 8
+        r[6] = -1.0
+        old = self.hist[-3:]
+        if self.counter != 1:
+            slot = self.appended % PLMS_RING
+            r[6] = float(slot)
+            self.hist = (old + [slot])[-PLMS_RING:]
+            self.appended += 1
+            weights = self.AB[len(old) + 1]
+        else:  # Heun restart: average with the first eps, from the sample the first step started at
+            prev, t = t, t + self.ratio
+            weights = (0.5, 0.5)
+            old = old[-1:]
+        a_t = self.alpha(t)
+        a_p = self.alpha(prev) if prev >= 0 else self.final_alpha
+        sc = math.sqrt(a_p / a_t)
+        k = (a_p - a_t) / (a_t * math.sqrt(1 - a_p) + math.sqrt(a_t * (1 - a_t) * a_p))
+        r[1 if self.counter == 1 else 0] = sc
+        r[7] = 1.0 if self.counter == 0 else 0.0
+        r[2] = -k * weights[0]
+        for w, s in zip(weights[1:], reversed(old)):  # weights[1] belongs to the newest remembered entry
+            r[3 + s] += -k * w
+        self.counter += 1
+        return r
+
+
+class PNDMScheduler(DDIMScheduler):
+    """diffusers `PNDMScheduler` with `skip_prk_steps=True` (PLMS), the scheduler the SD-1.5 inpainting checkpoint
+    stores and the v1 app samples with (reference app.py:91-93): N inference steps make N + 1 UNet evaluations, a
+    first Euler-like step, a Heun restart from the first step's sample (counter 1), then Adams-Bashforth of order
+    2, 3 and 4 on the guided eps. Restates diffusers 0.27.0 (schedulers/scheduling_pndm.py) as recalled from its
+    published source; oracle/pndm.py restates the same step by step. The Runge-Kutta warm-up (`skip_prk_steps=False`,
+    diffusers' default, used by no stored SD-1.x configuration) and v-prediction are not built.
+
+    Every step is linear in (x, the first step's sample, the new eps, up to 3 earlier eps), with weights that depend
+    on the step index only, so `plms_coefficients()` folds the schedule into one 8-float row per step (`_PlmsFold`)
+    and the arithmetic on the latents runs in the fused CFG + PLMS kernel (`pp_plms_step`)."""
+
+    order = 1
+    kind = "plms"
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, skip_prk_steps: bool = False,
+                 set_alpha_to_one: bool = False, prediction_type: str = "epsilon", timestep_spacing: str = "leading",
+                 steps_offset: int = 0, **unused):
+        if not skip_prk_steps:
+            raise NotImplementedError("skip_prk_steps=False (the Runge-Kutta warm-up) is not built: PLMS with "
+                                      "skip_prk_steps=True is, as stored by the SD-1.x checkpoints")
+        if prediction_type != "epsilon":
+            raise NotImplementedError(f"prediction_type={prediction_type!r}: only epsilon prediction is built")
+        if timestep_spacing not in ("linspace", "leading", "trailing"):
+            raise NotImplementedError(f"timestep_spacing={timestep_spacing!r}: linspace, leading and trailing are built")
+        super().__init__(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                         beta_schedule=beta_schedule, trained_betas=trained_betas, set_alpha_to_one=set_alpha_to_one,
+                         steps_offset=steps_offset, prediction_type=prediction_type, timestep_spacing=timestep_spacing)
+        self.config = _SchedConfig(
+            num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+            beta_schedule=beta_schedule, trained_betas=trained_betas, skip_prk_steps=skip_prk_steps,
+            set_alpha_to_one=set_alpha_to_one, prediction_type=prediction_type, timestep_spacing=timestep_spacing,
+            steps_offset=steps_offset)
+        self._state = None
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        c = self.config
+        T, n = c.num_train_timesteps, num_inference_steps
+        if n > T:
+            raise ValueError(f"`num_inference_steps`: {n} cannot be larger than `self.config.train_timesteps`: {T}")
+        self.num_inference_steps = n
+        if c.timestep_spacing == "linspace":
+            ts = np.linspace(0, T - 1, n).round().astype(np.int64)
+        elif c.timestep_spacing == "leading":
+            ts = (np.arange(0, n) * (T // n)).round().astype(np.int64) + c.steps_offset
+        else:
+            ts = np.round(np.arange(T, 0, -T / n))[::-1].astype(np.int64) - 1
+        # the last-but-one timestep is repeated: the Heun restart evaluates the net there a second time
+        plms = np.concatenate([ts[:-1], ts[-2:-1], ts[-1:]])[::-1].copy()
+        self.timesteps = torch.from_numpy(plms.astype(np.int64)).to(device)
+        self._state = None
+
+    def step_coefficients(self, timesteps=None, eta: float = 0.0) -> torch.Tensor:
+        """the shared 8-float rows (guidance / side-net scale / blend are filled in by the denoiser); DDIM columns
+        unused"""
+        n = len(self.timesteps if timesteps is None else timesteps)
+        return torch.zeros(n, 8, dtype=torch.float32)
+
+    def _fold(self) -> _PlmsFold:
+        ac = self.alphas_cumprod
+        return _PlmsFold(self.config.num_train_timesteps // self.num_inference_steps, lambda t: float(ac[t]),
+                         float(self.final_alpha_cumprod))
+
+    def plms_coefficients(self, first: int = 0, dtype=torch.float32) -> torch.Tensor:
+        """[len(timesteps) - first, 8] rows for `pp_plms_step` (folded in float64, returned as `dtype`), starting at
+        schedule index `first` (strength < 1 slices the schedule; the step counter and the history then start at 0
+        there, like diffusers' scheduler)"""
+        if self.num_inference_steps is None:
+            raise ValueError("call set_timesteps first")
+        fold = self._fold()
+        return torch.tensor([fold.row(t) for t in self.timesteps[first:].tolist()], dtype=dtype)
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True):
+        """eager x_t -> x_{t-1} on CUDA tensors through `pp_plms_step`; keeps diffusers' counter and eps history
+        (reset by `set_timesteps`)"""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after "
+                             "creating the scheduler")
+        if not sample.is_cuda:
+            raise RuntimeError("PNDMScheduler.step runs in the CUDA kernel pp_plms_step; CPU tensors are not "
+                               "supported (no CPU fallback on the hot path)")
+        from . import ops
+
+        nb, c, h, w = sample.shape
+        if c != 4:
+            raise ValueError("the fused step kernel handles 4-channel latents")
+        st = self._state
+        if st is None or st["shape"] != (nb, h, w) or st["device"] != sample.device:
+            z = lambda *s: torch.zeros(*s, nb, h * w, 4, dtype=torch.float32, device=sample.device)  # noqa: E731
+            st = self._state = dict(fold=self._fold() if st is None else st["fold"], shape=(nb, h, w),
+                                    device=sample.device, cur=z(), ets=z(PLMS_RING),
+                                    coef=torch.zeros(1, 8, device=sample.device))
+        row = torch.tensor([st["fold"].row(timestep)], dtype=torch.float32).to(sample.device)
+        lat = ops.nhwc_fp32_from_nchw(sample)
+        if lat.untyped_storage().data_ptr() == sample.untyped_storage().data_ptr():
+            lat = lat.clone()  # an fp32 channels_last sample: the kernel updates `lat` in place, never the caller's
+        eps = ops.nhwc_fp32_from_nchw(model_output)
+        ops.run(ops.plms_desc(eps=eps, eps_fp32=True, eps_ld=4, latents=lat, cur_sample=st["cur"], ets=st["ets"],
+                              coef=st["coef"], pcoef=row, step_idx=None, advance_step=False, do_cfg=False, batch=nb,
+                              hw=h * w))
+        prev = lat.view(nb, h, w, 4).permute(0, 3, 1, 2).contiguous().to(sample.dtype)
+        if not return_dict:
+            return (prev,)
+        return DDIMSchedulerOutput(prev_sample=prev)
