@@ -30,11 +30,13 @@ from types import SimpleNamespace
 from typing import Dict, List, Optional, Tuple
 
 import torch
-import torch.nn as nn
 
 from .. import _native as N
 from .. import ops
+from ..config import Config
 from ..engine import BF16, Plan, Pool, Recorder, _ceil
+from ..loading import rename_deprecated_vae_attention
+from .base import DiffusersModel
 
 
 # --------------------------------------------------------------------------- parameter layout
@@ -430,7 +432,7 @@ class DiagonalGaussianDistribution:
         return self.mean
 
 
-class AutoencoderKL(nn.Module):
+class AutoencoderKL(DiffusersModel):
     def __init__(self, in_channels: int = 3, out_channels: int = 3, latent_channels: int = 4,
                  block_out_channels: Tuple[int, ...] = (128, 256, 512, 512), layers_per_block: int = 2,
                  norm_num_groups: int = 32, scaling_factor: float = 0.18215, sample_size: int = 32):
@@ -439,10 +441,9 @@ class AutoencoderKL(nn.Module):
             raise NotImplementedError("the kernel path is built for RGB images and <= 4 latent channels (SD VAE)")
         if any(c % 8 for c in block_out_channels):
             raise ValueError("block_out_channels must be multiples of 8")
-        self.config = SimpleNamespace(in_channels=in_channels, out_channels=out_channels,
-                                      latent_channels=latent_channels, block_out_channels=tuple(block_out_channels),
-                                      layers_per_block=layers_per_block, scaling_factor=scaling_factor,
-                                      norm_num_groups=norm_num_groups, sample_size=sample_size)
+        self.config = Config(in_channels=in_channels, out_channels=out_channels, latent_channels=latent_channels,
+                             block_out_channels=tuple(block_out_channels), layers_per_block=layers_per_block,
+                             scaling_factor=scaling_factor, norm_num_groups=norm_num_groups, sample_size=sample_size)
         # tiled encode / decode, off by default (diffusers AutoencoderKL.__init__); the tile_* attributes may be set
         self.use_tiling = False
         self.use_slicing = False
@@ -453,56 +454,9 @@ class AutoencoderKL(nn.Module):
         for name, shape in vae_param_shapes(in_channels, out_channels, latent_channels, block_out_channels,
                                             layers_per_block).items():
             self._register(name, torch.zeros(shape))
-        self._engine: Optional[VaeEngine] = None
-        self._out_dtype = torch.float32
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
-    def _register(self, name: str, value: torch.Tensor):
-        parts = name.split(".")
-        mod = self
-        for p in parts[:-1]:
-            if not hasattr(mod, p):
-                mod.add_module(p, nn.Module())
-            mod = getattr(mod, p)
-        mod.register_parameter(parts[-1], nn.Parameter(value, requires_grad=False))
-
-    def _invalidate(self):
-        self._engine = None
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate()
-        return super()._apply(fn, *a, **k)
-
-    def to(self, *args, **kwargs):
-        # like the UNet: compute is always bf16 x bf16 -> fp32; a requested dtype only selects the output dtype
-        dtype = kwargs.pop("dtype", None)
-        rest = []
-        for a in args:
-            if isinstance(a, torch.dtype):
-                dtype = a
-            else:
-                rest.append(a)
-        if dtype is not None:
-            self._out_dtype = dtype
-        if not rest and not kwargs:
-            return self
-        return super().to(*rest, **kwargs)
-
-    @property
-    def dtype(self):
-        return self._out_dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
-    def engine(self) -> VaeEngine:
-        if self._engine is None:
-            dev = self.device
-            if dev.type != "cuda":
-                raise RuntimeError(f"AutoencoderKL must be on a CUDA device (got {dev}): there is no CPU path")
-            self._engine = VaeEngine(self.config, {k: v for k, v in self.state_dict().items()}, dev)
-        return self._engine
+    def _make_engine(self, state_dict, device) -> VaeEngine:
+        return VaeEngine(self.config, state_dict, device)
 
     # ---- tiling (diffusers AutoencoderKL.enable_tiling: opt-in, it blends tile seams and so changes the result)
     def enable_tiling(self, use_tiling: bool = True):
@@ -618,33 +572,13 @@ class AutoencoderKL(nn.Module):
                 "norm_num_groups", "scaling_factor", "sample_size")
         return cls(**{k: (tuple(config[k]) if isinstance(config[k], list) else config[k]) for k in keys if k in config})
 
-    @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path, subfolder: Optional[str] = None, torch_dtype=None,
-                        revision: Optional[str] = None, variant: Optional[str] = None, local_files_only: bool = False,
-                        cache_dir: Optional[str] = None, **unused) -> "AutoencoderKL":
-        """`config.json` + `diffusion_pytorch_model[.variant].safetensors | .bin`; the deprecated attention parameter
-        names of older VAE checkpoints (query / key / value / proj_attn) are renamed like diffusers does"""
-        from ..loading import load_json, load_weights, rename_deprecated_vae_attention, resolve_checkpoint_dir
-
-        d = resolve_checkpoint_dir(pretrained_model_name_or_path, subfolder, revision, local_files_only, cache_dir)
-        model = cls.from_config(load_json(d, "config.json"))
-        model.load_state_dict(rename_deprecated_vae_attention(load_weights(d, variant)), strict=True)
-        if torch_dtype is not None:
-            model.to(dtype=torch_dtype)
-        return model
-
-    def save_pretrained(self, save_directory, variant: Optional[str] = None, **unused):
-        import json
-        import os
-
-        from ..loading import save_weights
-
-        os.makedirs(save_directory, exist_ok=True)
+    def _diffusers_config(self) -> dict:
         cfg = {"_class_name": "AutoencoderKL", "_diffusers_version": "0.27.0", "act_fn": "silu"}
         cfg.update({k: (list(v) if isinstance(v, tuple) else v) for k, v in vars(self.config).items()})
-        with open(os.path.join(save_directory, "config.json"), "w") as f:
-            json.dump(cfg, f, indent=2, sort_keys=True)
-        save_weights(self.state_dict(), save_directory, variant=variant)
+        return cfg
+
+    # older VAE checkpoints name the attention parameters query / key / value / proj_attn: renamed like diffusers does
+    _checkpoint_state_dict = staticmethod(rename_deprecated_vae_attention)
 
     @classmethod
     def synthetic(cls, seed: int = 4321, tiny: bool = False, **kw) -> "AutoencoderKL":

@@ -18,13 +18,14 @@ from __future__ import annotations
 
 from collections import OrderedDict
 from types import SimpleNamespace
-from typing import Optional
 
 import torch
 import torch.nn as nn
 
 from .. import _native as N
+from ..config import Config
 from ..engine import BF16, Plan, Pool, Recorder
+from .base import KernelModule
 
 
 def clip_param_shapes(cfg) -> "OrderedDict[str, tuple]":
@@ -107,25 +108,21 @@ class ClipEngine(Recorder):
         return plan
 
 
-class _Container(nn.Module):
-    pass
-
-
-class CLIPTextModel(nn.Module):
+class CLIPTextModel(KernelModule):
     def __init__(self, vocab_size: int = 49408, hidden_size: int = 768, intermediate_size: int = 3072,
                  num_hidden_layers: int = 12, num_attention_heads: int = 12, max_position_embeddings: int = 77,
                  layer_norm_eps: float = 1e-5, hidden_act: str = "quick_gelu", **unused):
         super().__init__()
-        self.config = SimpleNamespace(vocab_size=vocab_size, hidden_size=hidden_size, intermediate_size=intermediate_size,
-                                      num_hidden_layers=num_hidden_layers, num_attention_heads=num_attention_heads,
-                                      max_position_embeddings=max_position_embeddings, layer_norm_eps=layer_norm_eps,
-                                      hidden_act=hidden_act)
+        self.config = Config(vocab_size=vocab_size, hidden_size=hidden_size, intermediate_size=intermediate_size,
+                             num_hidden_layers=num_hidden_layers, num_attention_heads=num_attention_heads,
+                             max_position_embeddings=max_position_embeddings, layer_norm_eps=layer_norm_eps,
+                             hidden_act=hidden_act)
         if hidden_size % num_attention_heads or hidden_size // num_attention_heads not in (8, 16, 32, 64):
             raise NotImplementedError("head dim must be 8, 16, 32 or 64")
         if max_position_embeddings > 128:
             raise NotImplementedError("at most 128 positions (CLIP: 77)")
-        self.text_model = _Container()
-        emb = self.text_model.embeddings = _Container()
+        self.text_model = nn.Module()
+        emb = self.text_model.embeddings = nn.Module()
         emb.token_embedding = nn.Embedding(vocab_size, hidden_size)
         emb.position_embedding = nn.Embedding(max_position_embeddings, hidden_size)
         for name, shape in clip_param_shapes(self.config).items():
@@ -134,43 +131,6 @@ class CLIPTextModel(nn.Module):
             self._register(name, torch.zeros(shape))
         for p in self.parameters():
             p.requires_grad_(False)
-        self._engine: Optional[ClipEngine] = None
-        self._out_dtype = torch.float32
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
-
-    def _register(self, name: str, value: torch.Tensor):
-        parts = name.split(".")
-        mod = self
-        for p in parts[:-1]:
-            if not hasattr(mod, p):
-                mod.add_module(p, _Container())
-            mod = getattr(mod, p)
-        mod.register_parameter(parts[-1], nn.Parameter(value, requires_grad=False))
-
-    def _invalidate(self):
-        self._engine = None
-
-    def _apply(self, fn, *a, **k):
-        self._invalidate()
-        return super()._apply(fn, *a, **k)
-
-    def to(self, *args, **kwargs):
-        dtype = kwargs.pop("dtype", None)
-        rest = []
-        for a in args:
-            if isinstance(a, torch.dtype):
-                dtype = a
-            else:
-                rest.append(a)
-        if dtype is not None:
-            self._out_dtype = dtype
-        if not rest and not kwargs:
-            return self
-        return super().to(*rest, **kwargs)
-
-    @property
-    def dtype(self):
-        return self._out_dtype
 
     @property
     def device(self):
@@ -195,17 +155,10 @@ class CLIPTextModel(nn.Module):
     def get_input_embeddings(self):
         return self.text_model.embeddings.token_embedding
 
-    def engine(self) -> ClipEngine:
-        if self._engine is None:
-            dev = self.device
-            if dev.type != "cuda":
-                raise RuntimeError(f"CLIPTextModel must be on a CUDA device (got {dev}): there is no CPU path")
-            sd = {}
-            for k, v in self.state_dict().items():
-                # EmbeddingLayerWithFixes keeps the base table under `.wrapped.weight`
-                sd[k.replace("token_embedding.wrapped.weight", "token_embedding.weight")] = v
-            self._engine = ClipEngine(self.config, sd, dev)
-        return self._engine
+    def _make_engine(self, state_dict, device) -> ClipEngine:
+        # EmbeddingLayerWithFixes keeps the base table under `.wrapped.weight`
+        sd = {k.replace("token_embedding.wrapped.weight", "token_embedding.weight"): v for k, v in state_dict.items()}
+        return ClipEngine(self.config, sd, device)
 
     # ---- the task-prompt splice, resolved to gather indices on the host
     def _gather_plan(self, input_ids: torch.Tensor):

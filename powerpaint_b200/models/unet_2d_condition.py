@@ -17,14 +17,16 @@ reference does (unet_2d_condition.py:1223); outputs are fresh tensors in `self.d
 from __future__ import annotations
 
 from dataclasses import asdict, dataclass
-from types import SimpleNamespace
 from typing import Any, Dict, List, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
 
 from .. import ops
+from ..config import Config
 from ..engine import NetConfig, NetEngine, guess_mode_alphas
+from ..loading import net_config_from_diffusers, net_config_to_diffusers
+from .base import DiffusersModel
 from .spec import param_shapes, synthetic_state_dict
 
 
@@ -46,20 +48,7 @@ class ControlNetOutput:
     mid_block_res_sample: torch.Tensor
 
 
-class _Config(SimpleNamespace):
-    """attribute + mapping access like diffusers' FrozenDict config"""
-
-    def __getitem__(self, k):
-        return getattr(self, k)
-
-    def __contains__(self, k):
-        return hasattr(self, k)
-
-    def get(self, k, default=None):
-        return getattr(self, k, default)
-
-
-def _make_config(cfg: NetConfig, **extra) -> _Config:
+def _make_config(cfg: NetConfig, **extra) -> Config:
     d = asdict(cfg)
     d.update(dict(sample_size=extra.pop("sample_size", 64), time_cond_proj_dim=None, flip_sin_to_cos=True,
                   freq_shift=0, act_fn="silu", use_linear_projection=False, only_cross_attention=False,
@@ -76,10 +65,10 @@ def _make_config(cfg: NetConfig, **extra) -> _Config:
                   reverse_transformer_layers_per_block=None, time_embedding_act_fn=None, time_embedding_dim=None,
                   time_embedding_type="positional", timestep_post_act=None, transformer_layers_per_block=1))
     d.update(extra)
-    return _Config(**d)
+    return Config(**d)
 
 
-class _HotPathModel(nn.Module):
+class _HotPathModel(DiffusersModel):
     KIND = "unet"
 
     def __init__(self, cfg: Optional[NetConfig] = None, sample_size: int = 64, **cfg_kwargs):
@@ -88,34 +77,8 @@ class _HotPathModel(nn.Module):
             cfg = NetConfig(**cfg_kwargs)
         self._cfg = cfg
         self.config = _make_config(cfg, sample_size=sample_size)
-        self._out_dtype = torch.float32
         for name, shape in param_shapes(cfg, self.KIND).items():
             self._register(name, torch.zeros(shape))
-        self._engine: Optional[NetEngine] = None
-        self._generation = 0  # bumped whenever the parameters change: recorded programs of older engines are stale
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
-
-    # ---- parameter tree with diffusers names
-    def _register(self, name: str, value: torch.Tensor):
-        parts = name.split(".")
-        mod = self
-        for p in parts[:-1]:
-            if not hasattr(mod, p):
-                mod.add_module(p, nn.Module())
-            mod = getattr(mod, p)
-        mod.register_parameter(parts[-1], nn.Parameter(value, requires_grad=False))
-
-    def _invalidate(self):
-        self._engine = None
-        self._generation += 1
-
-    @property
-    def generation(self) -> int:
-        return self._generation
-
-    def _apply(self, fn, *a, **k):  # .to() / .cuda() / .half() move parameters: repack lazily
-        self._invalidate()
-        return super()._apply(fn, *a, **k)
 
     @classmethod
     def from_state_dict(cls, cfg: NetConfig, state_dict: Dict[str, torch.Tensor], **kw):
@@ -127,77 +90,21 @@ class _HotPathModel(nn.Module):
     def synthetic(cls, cfg: NetConfig, seed: int = 1234, **kw):
         return cls.from_state_dict(cfg, synthetic_state_dict(cfg, cls.KIND, seed), **kw)
 
+    def _make_engine(self, state_dict, device) -> NetEngine:
+        return NetEngine(self._cfg, state_dict, self.KIND, device)
+
     # ---- checkpoint directories in the diffusers layout (ref:app.py:121-123,141-147,165-171)
     @classmethod
     def from_config(cls, config, **kw):
         """a diffusers `config.json` dictionary (or another model's `.config`) -> an uninitialised model"""
-        from ..loading import net_config_from_diffusers
-
         d = dict(vars(config)) if not isinstance(config, dict) else dict(config)
         m = cls(net_config_from_diffusers(d, cls.KIND), sample_size=d.get("sample_size") or 64, **kw)
         if cls.KIND != "unet":
             m.config.global_pool_conditions = bool(d.get("global_pool_conditions", False))
         return m
 
-    @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path, subfolder: Optional[str] = None, torch_dtype=None,
-                        revision: Optional[str] = None, variant: Optional[str] = None, local_files_only: bool = False,
-                        cache_dir: Optional[str] = None, **unused):
-        """`ModelMixin.from_pretrained` for a local directory or a cached hub snapshot: `config.json` +
-        `diffusion_pytorch_model[.variant].safetensors | .bin`, strict load, on the CPU. `torch_dtype` selects the
-        dtype of returned tensors (compute is bf16 x bf16 -> fp32 whatever it says)."""
-        from ..loading import load_json, load_weights, resolve_checkpoint_dir
-
-        d = resolve_checkpoint_dir(pretrained_model_name_or_path, subfolder, revision, local_files_only, cache_dir)
-        model = cls.from_config(load_json(d, "config.json"))
-        model.load_state_dict(load_weights(d, variant), strict=True)
-        if torch_dtype is not None:
-            model.to(dtype=torch_dtype)
-        return model
-
-    def save_pretrained(self, save_directory, variant: Optional[str] = None, **unused):
-        import json
-        import os
-
-        from ..loading import net_config_to_diffusers, save_weights
-
-        os.makedirs(save_directory, exist_ok=True)
-        with open(os.path.join(save_directory, "config.json"), "w") as f:
-            json.dump(net_config_to_diffusers(self._cfg, self.KIND, self.config), f, indent=2, sort_keys=True)
-        save_weights(self.state_dict(), save_directory, variant=variant)
-
-    # ---- diffusers-like surface
-    @property
-    def dtype(self) -> torch.dtype:
-        return self._out_dtype
-
-    @property
-    def device(self) -> torch.device:
-        return next(self.parameters()).device
-
-    def to(self, *args, **kwargs):
-        # the reference app calls unet.to(dtype=fp16); compute is always bf16 x bf16 -> fp32 here,
-        # the requested dtype only selects the dtype of returned tensors
-        dtype = kwargs.get("dtype")
-        for a in args:
-            if isinstance(a, torch.dtype):
-                dtype = a
-        if dtype is not None:
-            self._out_dtype = dtype
-            kwargs.pop("dtype", None)
-            args = tuple(a for a in args if not isinstance(a, torch.dtype))
-            if not args and not kwargs:
-                return self
-        return super().to(*args, **kwargs)
-
-    def engine(self) -> NetEngine:
-        if self._engine is None:
-            dev = self.device
-            if dev.type != "cuda":
-                raise RuntimeError(f"{type(self).__name__} must be on a CUDA device (got {dev}); "
-                                   "the hot path has no CPU fallback")
-            self._engine = NetEngine(self._cfg, {k: v for k, v in self.state_dict().items()}, self.KIND, dev)
-        return self._engine
+    def _diffusers_config(self) -> dict:
+        return net_config_to_diffusers(self._cfg, self.KIND, self.config)
 
     # ---- shared helpers
     @staticmethod

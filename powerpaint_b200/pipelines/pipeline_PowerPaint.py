@@ -18,9 +18,13 @@ from typing import Callable, List, Optional, Union
 import torch
 
 from ..denoise import FusedDenoiser
-from ..models.unet_2d_condition import UNet2DConditionModel
+from ..models import AutoencoderKL, BrushNetModel, ControlNetModel, UNet2DConditionModel
 from .common import (StableDiffusionPipelineOutput, callback_fires, decode_latents, encode_text,
                      prepare_mask_and_masked_image, randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
+
+# the components stored as diffusers model directories, by their name in model_index.json
+_MODEL_COMPONENTS = {"unet": UNet2DConditionModel, "brushnet": BrushNetModel, "controlnet": ControlNetModel,
+                     "vae": AutoencoderKL}
 
 
 class StableDiffusionInpaintPipeline:
@@ -100,18 +104,11 @@ class StableDiffusionInpaintPipeline:
     def _load_component(name: str, directory: str, entry, torch_dtype, variant):
         """one subfolder of a pipeline directory; `entry` = [library, class name] of model_index.json"""
         from ..loading import load_json
-        from ..models import AutoencoderKL, BrushNetModel, ControlNetModel
         from .. import schedulers
         from ..schedulers import DDIMScheduler
 
-        if name == "unet":
-            return UNet2DConditionModel.from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
-        if name == "brushnet":
-            return BrushNetModel.from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
-        if name == "controlnet":
-            return ControlNetModel.from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
-        if name == "vae":
-            return AutoencoderKL.from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
+        if name in _MODEL_COMPONENTS:
+            return _MODEL_COMPONENTS[name].from_pretrained(directory, torch_dtype=torch_dtype, variant=variant)
         if name in ("text_encoder", "text_encoder_brushnet"):
             import transformers
 

@@ -19,19 +19,7 @@ from typing import List, Optional, Tuple, Union
 import numpy as np
 import torch
 
-
-class _SchedConfig(SimpleNamespace):
-    def __getitem__(self, k):
-        return getattr(self, k)
-
-    def __contains__(self, k):
-        return hasattr(self, k)
-
-    def get(self, k, default=None):
-        return getattr(self, k, default)
-
-    def keys(self):
-        return self.__dict__.keys()
+from .config import Config
 
 
 class DDIMSchedulerOutput(SimpleNamespace):
@@ -52,7 +40,7 @@ class DDIMScheduler:
             raise NotImplementedError("only prediction_type='epsilon' is on the PowerPaint hot path")
         if clip_sample or thresholding or rescale_betas_zero_snr:
             raise NotImplementedError("clip_sample / thresholding / zero-SNR rescale are off in the SD config")
-        self.config = _SchedConfig(
+        self.config = Config(
             num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
             beta_schedule=beta_schedule, trained_betas=trained_betas, clip_sample=clip_sample,
             set_alpha_to_one=set_alpha_to_one, steps_offset=steps_offset, prediction_type=prediction_type,
@@ -398,7 +386,7 @@ class _SolverScheduler(DDIMScheduler):
                          beta_schedule=beta_schedule, trained_betas=trained_betas, prediction_type=prediction_type,
                          thresholding=thresholding, timestep_spacing=timestep_spacing, steps_offset=steps_offset,
                          rescale_betas_zero_snr=rescale_betas_zero_snr)
-        self.config = _SchedConfig(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+        self.config = Config(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
                                    beta_schedule=beta_schedule, trained_betas=trained_betas,
                                    prediction_type=prediction_type, thresholding=thresholding,
                                    timestep_spacing=timestep_spacing, steps_offset=steps_offset,
@@ -810,7 +798,7 @@ class PNDMScheduler(DDIMScheduler):
         super().__init__(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
                          beta_schedule=beta_schedule, trained_betas=trained_betas, set_alpha_to_one=set_alpha_to_one,
                          steps_offset=steps_offset, prediction_type=prediction_type, timestep_spacing=timestep_spacing)
-        self.config = _SchedConfig(
+        self.config = Config(
             num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
             beta_schedule=beta_schedule, trained_betas=trained_betas, skip_prk_steps=skip_prk_steps,
             set_alpha_to_one=set_alpha_to_one, prediction_type=prediction_type, timestep_spacing=timestep_spacing,
