@@ -231,8 +231,9 @@ typedef struct pp_gn_desc {
     float eps;
     int32_t silu;
     float* stats; /* scratch of pp_group_norm_scratch_bytes() bytes, 16-byte aligned: the per-(sample, group)
-                     sum / sum of squares [batch, groups, 2] fp32, then the ticket counters and per-block
-                     partials of the deterministic reduction */
+                     (mean, rstd) [batch, groups, 2] fp32 both statistics paths write, then (standalone path,
+                     at the next 16-byte boundary) the ticket counters [batch] uint32 and, again 16-byte
+                     aligned, the per-block partials of the deterministic reduction */
     void* y;
     int32_t stats_prezeroed; /* 1: the scratch was zeroed once when it was allocated (every call leaves its
                                 ticket counters zero again) or by one memset per step over all scratch;

@@ -1008,7 +1008,26 @@ class _Census:
         self.counts[source] = self.counts.get(source, 0) + 1
 
 
-def _capture_all(monkeypatch, census):
+# the Program record methods besides `add` (which takes a descriptor): a census sees each call as a `ProgramCall`
+PROGRAM_RECORD_METHODS = ("add_layer_norm", "add_upsample2x", "add_upsample_nearest", "add_softmax_rows",
+                          "add_embed_gather", "add_causal_attention_small", "add_add", "add_time_embed",
+                          "add_window_copy", "add_memset")
+
+
+class ProgramCall:
+    """one Program.add_<kind>(...) call: `kind` and the bound arguments by parameter name"""
+
+    def __init__(self, kind, args):
+        self.kind = kind
+        self.args = args
+
+
+def _capture_all(monkeypatch, census, tiled_vae=False):
+    """record the production programs (the denoisers under every engine switch, VAE encode / decode at 512^2, the
+    text encoder; `tiled_vae`: also a tiled VAE decode) and hand every recorded op to census.record(source, op): a
+    Desc for Program.add, a ProgramCall for the other record methods"""
+    import inspect
+
     from powerpaint_b200 import ops as o
     from powerpaint_b200.denoise import FusedDenoiser
     from powerpaint_b200.engine import NetConfig, Recorder
@@ -1022,6 +1041,15 @@ def _capture_all(monkeypatch, census):
         census.record(source[0], desc)
         return orig_add(self, desc)
     monkeypatch.setattr(o.Program, "add", add)
+    originals = {}
+    for meth in PROGRAM_RECORD_METHODS:
+        originals[meth] = orig = getattr(o.Program, meth)
+
+        def hook(self, *args, _orig=orig, _kind=meth[len("add_"):], **kw):
+            bound = inspect.signature(_orig).bind(self, *args, **kw).arguments
+            census.record(source[0], ProgramCall(_kind, {k: v for k, v in bound.items() if k != "self"}))
+            return _orig(self, *args, **kw)
+        monkeypatch.setattr(o.Program, meth, hook)
     dev = _dev()
     u9 = UNet2DConditionModel.synthetic(NetConfig(in_channels=9), seed=1234).to(dev)
     u4 = UNet2DConditionModel.synthetic(NetConfig(in_channels=4), seed=1234).to(dev)
@@ -1053,6 +1081,10 @@ def _capture_all(monkeypatch, census):
     vae.engine().encode_plan(1, 512, 512)
     source[0] = "VAE decode 512x512"
     vae.engine().decode_plan(1, 64, 64)
+    if tiled_vae:  # the SD checkpoint's tile sizes: an 80 x 80 latent decodes as 2 x 2 overlapping 64 x 64 tiles
+        vae.tile_sample_min_size, vae.tile_latent_min_size = 512, 64
+        source[0] = "VAE tiled decode 80x80"
+        vae.engine().tiled_plan(False, 1, 80, 80, vae.tile_geometry(False, 80, 80), vae._tiling_key())
     del vae
     te = CLIPTextModel().to(dev)
     source[0] = "text encoder 2x77"
@@ -1060,6 +1092,8 @@ def _capture_all(monkeypatch, census):
     del te
     torch.cuda.empty_cache()
     monkeypatch.setattr(o.Program, "add", orig_add)
+    for meth, orig in originals.items():
+        monkeypatch.setattr(o.Program, meth, orig)
 
 
 def _fresh_gemm(c0, variant, seed):

@@ -283,15 +283,7 @@ def test_small_ops(ops):
     assert (zn[..., 9:] == 0).all()
     back = ops.nhwc_to_nchw(zn, 9)
     assert torch.equal(back, z.to(BF16).float())
-    # timestep embedding
-    t = torch.tensor([981.0, 1.0, 500.0], device=_dev())
-    e = torch.zeros(3, 320, device=_dev(), dtype=BF16)
-    ops.time_embed(t, e)
-    half = 160
-    f = torch.exp(-math.log(10000.0) * torch.arange(half, device=_dev(), dtype=torch.float32) / half)
-    arg = t[:, None] * f[None]
-    ref = torch.cat([torch.cos(arg), torch.sin(arg)], -1)
-    assert (e.float() - ref).abs().max().item() < 1e-2
+    # the timestep embedding is checked per element against fp64 in test_norm_and_small_kernels_gpu.py
     torch.cuda.synchronize()
 
 
