@@ -119,6 +119,12 @@ int cfg_ddim_validate(const pp_cfg_ddim_desc& d) {
     PP_REQUIRE(!d.advance_step || d.step_idx, "cfg_ddim: advance_step needs step_idx");
     PP_REQUIRE((d.blend_x0 == nullptr) == (d.blend_mask == nullptr) && (d.blend_x0 == nullptr) == (d.blend_noise == nullptr),
                "cfg_ddim: blend_x0 / blend_mask / blend_noise go together");
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(d.latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.noise) & 15) == 0,
+               "cfg_ddim: latents / noise need 16-byte alignment");
+    PP_REQUIRE(!(d.eps_fp32 && d.eps_ld == 4) || (reinterpret_cast<uintptr_t>(d.eps) & 15) == 0,
+               "cfg_ddim: fp32 eps with eps_ld 4 needs 16-byte alignment");
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(d.blend_x0) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.blend_noise) & 15) == 0,
+               "cfg_ddim: blend_x0 / blend_noise need 16-byte alignment");
     if (d.next_in) {
         PP_REQUIRE(d.next_c >= 4 && d.n_copies >= 1, "cfg_ddim: next_in needs next_c >= 4, n_copies >= 1");
         PP_REQUIRE(d.extra_c == 0 || d.extra, "cfg_ddim: extra_c without extra");
@@ -208,6 +214,11 @@ int unipc_validate(const pp_unipc_desc& d) {
     PP_REQUIRE(d.eps && d.latents && d.last_sample && d.m1 && d.m2 && d.coef && d.ucoef, "unipc: null pointer");
     PP_REQUIRE(d.batch > 0 && d.hw > 0 && d.eps_ld >= 4, "unipc: invalid shape");
     PP_REQUIRE(!d.advance_step || d.step_idx, "unipc: advance_step needs step_idx");
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(d.latents) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.last_sample) & 15) == 0 &&
+                   (reinterpret_cast<uintptr_t>(d.m1) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.m2) & 15) == 0,
+               "unipc: latents / last_sample / m1 / m2 need 16-byte alignment");
+    PP_REQUIRE(!(d.eps_fp32 && d.eps_ld == 4) || (reinterpret_cast<uintptr_t>(d.eps) & 15) == 0,
+               "unipc: fp32 eps with eps_ld 4 needs 16-byte alignment");
     if (d.next_in)
         PP_REQUIRE(d.next_c >= 4 && d.next_c % 4 == 0 && d.n_copies >= 1 && (reinterpret_cast<uintptr_t>(d.next_in) & 7) == 0,
                    "unipc: next_in needs next_c %% 4 == 0, n_copies >= 1 and 8-byte alignment");

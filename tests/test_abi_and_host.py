@@ -48,6 +48,53 @@ def test_invalid_descriptors_fail_loudly_without_gpu():
     with pytest.raises(RuntimeError):
         N.check(1, "x")
 
+    # the step kernels move latents, state, noise, blend inputs and fp32 eps (eps_ld 4) as float4: a view one float
+    # off a 16-byte boundary must be refused when it is recorded. Integer addresses only: recording validates and
+    # launches nothing.
+    base = 1 << 20
+
+    def refused(add, desc, what):
+        prog = N.vp()
+        N.check(L.pp_program_create(ctypes.byref(prog)), "pp_program_create")
+        try:
+            rc = add(prog, ctypes.byref(desc))
+            return rc != 0 and what in L.pp_last_error()
+        finally:
+            L.pp_program_destroy(prog)
+
+    def ddim(**kw):
+        d = N.CfgDdimDesc()
+        d.eps, d.eps_fp32, d.eps_ld = base, 1, 4
+        d.latents, d.coef, d.batch, d.hw, d.do_cfg = base + 4096, base + 8192, 1, 64, 1
+        for k, v in kw.items():
+            setattr(d, k, v)
+        return d
+
+    def unipc(**kw):
+        d = N.UniPCDesc()
+        d.eps, d.eps_fp32, d.eps_ld = base, 1, 4
+        d.latents, d.last_sample, d.m1, d.m2 = base + 4096, base + 8192, base + 12288, base + 16384
+        d.coef, d.ucoef, d.batch, d.hw, d.do_cfg = base + 20480, base + 24576, 1, 64, 1
+        for k, v in kw.items():
+            setattr(d, k, v)
+        return d
+
+    assert not refused(L.pp_program_add_cfg_ddim, ddim(), b"cfg_ddim"), L.pp_last_error()
+    assert not refused(L.pp_program_add_cfg_ddim, ddim(eps=base + 4, eps_fp32=0), b"cfg_ddim")  # bf16 eps: scalar loads
+    assert not refused(L.pp_program_add_cfg_ddim, ddim(eps=base + 4, eps_ld=8), b"cfg_ddim")    # strided eps: scalar
+    blend = dict(blend_x0=base + 32768, blend_mask=base + 36868, blend_noise=base + 40960)    # the mask is read per float
+    assert not refused(L.pp_program_add_cfg_ddim, ddim(**blend), b"cfg_ddim"), L.pp_last_error()
+    for field in ("latents", "noise", "eps"):
+        assert refused(L.pp_program_add_cfg_ddim, ddim(**{field: (getattr(ddim(), field) or base + 49152) + 4}),
+                       b"cfg_ddim"), field
+    for field in ("blend_x0", "blend_noise"):
+        assert refused(L.pp_program_add_cfg_ddim, ddim(**blend | {field: blend[field] + 4}), b"cfg_ddim"), field
+    assert not refused(L.pp_program_add_unipc, unipc(), b"unipc"), L.pp_last_error()
+    assert not refused(L.pp_program_add_unipc, unipc(eps=base + 4, eps_fp32=0), b"unipc")
+    assert not refused(L.pp_program_add_unipc, unipc(eps=base + 4, eps_ld=8), b"unipc")
+    for field in ("latents", "last_sample", "m1", "m2", "eps"):
+        assert refused(L.pp_program_add_unipc, unipc(**{field: getattr(unipc(), field) + 4}), b"unipc"), field
+
 
 def test_group_norm_scratch_size_is_a_pure_host_query():
     from powerpaint_b200 import ops

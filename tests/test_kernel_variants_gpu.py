@@ -91,6 +91,45 @@ def gemm_out_geometry(d):
     return d.nb * ho * wo, ho, wo
 
 
+def gemm_extents(d):
+    """{pointer field: (rows, elements per row, row pitch in elements, dtype)} of every operand and output a descriptor
+    reads or writes, as include/powerpaint_b200.h defines them (GEMM N columns before the GEGLU pairing)"""
+    from powerpaint_b200 import _native as nat
+
+    M, _, _ = gemm_out_geometry(d)
+    N = d.N
+    e = {}
+    if d.a_mode:
+        e["a0"] = (d.nb * d.h * d.w, d.c0, d.c0, BF16)
+        if d.a1:
+            e["a1"] = (d.nb * d.h * d.w, d.c1, d.c1, BF16)
+    else:
+        e["a0"] = (M, d.c0, d.lda0, BF16)
+        if d.a1:
+            e["a1"] = (M, d.c1, d.lda1, BF16)
+    packed = d.a_mode != 0 or bool(d.a1)
+    kw = (9 if d.a_mode else 1) * ((d.c0 + 63) // 64 * 64 + ((d.c1 + 63) // 64 * 64 if d.a1 else 0)) if packed \
+        else d.c0
+    e["b"] = (N, kw, kw if packed else d.ldb, BF16)
+    e["bias"] = (1, N, N, torch.float32)
+    if d.rowvec:
+        e["rowvec"] = (d.nb if d.a_mode else (M + d.rows_per_group - 1) // d.rows_per_group, N, d.rowvec_ld or N,
+                       torch.float32)
+    e["res1"], e["res2"] = (M, N, d.ldr1, BF16), (M, N, d.ldr2, BF16)
+    e["ln_stats"], e["ln_u"] = (M, 2, 2, torch.float32), (1, N, N, torch.float32)
+    if d.epilogue == nat.PP_EPI_GEGLU:
+        e["out"] = (M, N // 2, d.ldc, BF16)
+    elif d.epilogue == nat.PP_EPI_TRANSPOSED:
+        e["out"] = (M // d.t_rows * N, d.t_rows, d.t_ld, F16 if d.t_fp16 else BF16)
+    elif d.epilogue == nat.PP_EPI_ROWS_THEN_TRANSPOSED:
+        tfc = d.trans_from_col
+        e["out"] = (M, tfc, d.ldc, BF16)
+        e["out_t"] = (M // d.t_rows * (N - tfc), d.t_rows, d.t_ld, F16 if d.t_fp16 else BF16)
+    else:
+        e["out"] = (M, N, d.ldc, torch.float32 if d.out_fp32 else BF16)
+    return {k: v for k, v in e.items() if getattr(d, k)}
+
+
 def _acc_chunk(d, t, r0, r1):
     """fp64 A W^T and |A| |W|^T for output rows [r0, r1) (conv chunks: whole samples)"""
     pad = lambda c: (c + 63) // 64 * 64  # noqa: E731
@@ -1116,18 +1155,15 @@ def _fresh_gemm(c0, variant, seed):
         if d.a1:
             t["a1"] = _nan_padded(M, d.c1, d.lda1, BF16, g)
     taps = 9 if d.a_mode else 1
+    ext = gemm_extents(d)
     if taps == 9 or d.a1:
-        p0 = (d.c0 + 63) // 64 * 64
-        p1 = (d.c1 + 63) // 64 * 64 if d.a1 else 0
-        t["b"] = (torch.randn(N, taps * (p0 + p1), device=_dev(), generator=g)
-                  / math.sqrt(taps * (d.c0 + d.c1))).to(BF16)
+        t["b"] = (torch.randn(N, ext["b"][1], device=_dev(), generator=g) / math.sqrt(taps * (d.c0 + d.c1))).to(BF16)
     else:
         t["b"] = _nan_padded(N, d.c0, d.ldb, BF16, g, 1 / math.sqrt(d.c0))
     if d.bias:
         t["bias"] = torch.randn(N, device=_dev(), generator=g)
     if d.rowvec:
-        groups = d.nb if d.a_mode else (M + d.rows_per_group - 1) // d.rows_per_group
-        ld = d.rowvec_ld or N
+        groups, _, ld, _ = ext["rowvec"]
         mis = (c0.rowvec & 15) // 4  # keep the production pointer's 16-byte misalignment (it selects the epilogue)
         buf = torch.full((groups * ld + 8,), float("nan"), device=_dev())
         t["rowvec"] = buf[mis:]

@@ -287,33 +287,184 @@ def test_small_ops(ops):
     torch.cuda.synchronize()
 
 
+U32 = 2.0 ** -24  # unit round-off of fp32
+
+
+def _cfg_eps(eps, gscale, do_cfg, B):
+    """(eps after CFG, |eps| magnitude of the terms) in fp64 from the stored eps rows (channels 0..3)"""
+    e = eps.double()
+    if not do_cfg:
+        return e[:B], e[:B].abs()
+    u, c = e[:B], e[B:2 * B]
+    return u + gscale * (c - u), u.abs() + abs(gscale) * (c.abs() + u.abs())
+
+
+def ref_cfg_ddim(eps, x, noise, cf, gscale, do_cfg, B, blend=None):
+    """fp64 evaluation of the pp_cfg_ddim_desc row formula (include/powerpaint_b200.h) on the stored fp32 inputs:
+    (x_prev, bound). The bound is a few fp32 round-offs of the sum of the magnitudes of every term, the most an fp32
+    evaluation of the same expression (with or without FMA contraction) can be off."""
+    cf = [float(v) for v in cf]
+    e, ea = _cfg_eps(eps, gscale, do_cfg, B)
+    xd = x.double()
+    inv = 1.0 / cf[0]
+    x0 = (xd - cf[1] * e) * inv
+    x0a = (xd.abs() + abs(cf[1]) * ea) * abs(inv)
+    nz = noise.double() if noise is not None else torch.zeros_like(xd)
+    xp = cf[2] * x0 + cf[3] * e + cf[4] * nz
+    xpa = abs(cf[2]) * x0a + abs(cf[3]) * ea + abs(cf[4]) * nz.abs()
+    if blend is not None:
+        o, m, nn = (t.double() for t in blend)
+        m = m.reshape(1, -1, 1)
+        a = cf[7]
+        s1a = max(1 - a * a, 0.0) ** 0.5
+        xp = (1 - m) * (a * o[None] + s1a * nn) + m * xp
+        # sqrtf(1 - a*a) is off by about u / (1 - a^2) relative: a < 0.95 keeps that within the factor below
+        xpa = (1 - m).abs() * (abs(a) * o[None].abs() + s1a * nn.abs()) * 16 + m.abs() * xpa
+    return xp, 12 * U32 * xpa + 1e-30
+
+
+def ref_unipc(eps, x, last, m1, m2, u, gscale, do_cfg, B):
+    """fp64 evaluation of the pp_unipc_desc row formula: (x_next, x_c, m_t, bound of each)"""
+    u = [float(v) for v in u]
+    e, ea = _cfg_eps(eps, gscale, do_cfg, B)
+    xd, ld, a1, a2 = x.double(), last.double(), m1.double(), m2.double()
+    mt = u[0] * xd + u[1] * e
+    mta = abs(u[0]) * xd.abs() + abs(u[1]) * ea
+    if u[2] != 0:
+        xc = u[3] * ld + u[4] * a1 + u[5] * a2 + u[6] * mt
+        xca = abs(u[3]) * ld.abs() + abs(u[4]) * a1.abs() + abs(u[5]) * a2.abs() + abs(u[6]) * mta
+    else:
+        xc, xca = xd, xd.abs() * 0
+    xn = u[7] * xc + u[8] * mt + u[9] * a1
+    xna = abs(u[7]) * (xca + xc.abs()) + abs(u[8]) * mta + abs(u[9]) * a1.abs()
+    b = lambda mag: 12 * U32 * mag + 1e-30  # noqa: E731
+    return xn, xc, mt, b(xna), b(xca), b(mta)
+
+
+def _eps_input(kind, nb, hw, g):
+    """(tensor the kernel reads, eps_fp32, eps_ld, channels 0..3 as the kernel sees them)"""
+    if kind == "fp32_vec":
+        e = torch.randn(nb, hw, 4, device=_dev(), generator=g)
+        return e, True, 4, e
+    if kind == "fp32_strided":
+        e = torch.randn(nb, hw, 8, device=_dev(), generator=g)
+        return e, True, 8, e[..., :4]
+    e = torch.randn(nb, hw, 8, device=_dev(), generator=g).to(BF16)
+    return e, False, 8, e[..., :4].float()
+
+
+def _within(got, ref, bound):
+    return bool(((got.double() - ref).abs() <= bound).all())
+
+
 def test_cfg_ddim(ops):
-    B, hw = 3, 64 * 64
+    """pp_cfg_ddim_step against the fp64 row formula to an fp32 round-off bound, per element; next_in equal to the bf16
+    rounding of the stored latents bit for bit, the extra channels to bf16 of `extra` (one set per copy with
+    extra_per_copy) followed by zeros, and channels 4 and up untouched without extra"""
+    for case in ("cfg_extra", "no_cfg", "bf16_strided", "fp32_strided", "guidance_from_coef", "extra_per_copy", "blend",
+                 "latents_only"):
+        _cfg_ddim_case(ops, case)
+
+
+def _cfg_ddim_case(ops, case):
+    B, hw, C = 3, 37 * 13, 16
     g = torch.Generator(device="cuda").manual_seed(9)
-    eps = torch.randn(2 * B, hw, 4, device=_dev(), generator=g)
+    do_cfg = case != "no_cfg"
+    nb = 2 * B if do_cfg else B
+    eps, eps_fp32, eps_ld, eps_view = _eps_input({"bf16_strided": "bf16_strided", "fp32_strided": "fp32_strided"}
+                                                 .get(case, "fp32_vec"), nb, hw, g)
     lat = torch.randn(B, hw, 4, device=_dev(), generator=g)
-    extra = torch.randn(B, hw, 5, device=_dev(), generator=g)
-    noise = torch.randn(B, hw, 4, device=_dev(), generator=g)
+    n_copies = 2 if do_cfg else 1
+    extra_c = 0 if case in ("blend", "latents_only") else 5
+    extra = torch.randn((n_copies if case == "extra_per_copy" else 1) * B, hw, 5, device=_dev(), generator=g)
+    noise = torch.randn(B, hw, 4, device=_dev(), generator=g) if case != "blend" else None
     a_t, a_p, sigma = 0.3, 0.45, 0.1
-    coef = torch.tensor([[0] * 8, [math.sqrt(a_t), math.sqrt(1 - a_t), math.sqrt(a_p),
-                                   math.sqrt(1 - a_p - sigma ** 2), sigma, 0, 0, 0]], device=_dev(), dtype=torch.float32)
+    row = [math.sqrt(a_t), math.sqrt(1 - a_t), math.sqrt(a_p), math.sqrt(1 - a_p - sigma ** 2), sigma, 3.25, 0, 0.7]
+    coef = torch.tensor([[float("nan")] * 8, row], device=_dev(), dtype=torch.float32)
+    gscale = 3.25 if case == "guidance_from_coef" else 7.5
+    blend = None
+    if case == "blend":
+        blend = (torch.randn(hw, 4, device=_dev(), generator=g), torch.rand(hw, device=_dev(), generator=g),
+                 torch.randn(B, hw, 4, device=_dev(), generator=g))
+        blend[1][: hw // 2] = (blend[1][: hw // 2] > 0.5).float()  # the production mask is binary; the rest is not
     step = torch.tensor([1], device=_dev(), dtype=torch.int32)
-    nxt = torch.full((2 * B, hw, 16), float("nan"), device=_dev(), dtype=BF16)
+    nxt = torch.full((n_copies * B, hw, C), float("nan"), device=_dev(), dtype=BF16)
     lat_in = lat.clone()
-    ops.run(ops.cfg_ddim_desc(eps=eps, eps_fp32=True, eps_ld=4, latents=lat, coef=coef, step_idx=step,
-                              advance_step=True, noise=noise, guidance_scale=7.5, do_cfg=True, batch=B, hw=hw,
-                              next_in=nxt, next_c=16, n_copies=2, extra=extra, extra_c=5))
+    ops.run(ops.cfg_ddim_desc(eps=eps, eps_fp32=eps_fp32, eps_ld=eps_ld, latents=lat, coef=coef, step_idx=step,
+                              advance_step=True, noise=noise, guidance_scale=0.0 if case == "guidance_from_coef" else 7.5,
+                              guidance_from_coef=case == "guidance_from_coef", do_cfg=do_cfg, batch=B, hw=hw,
+                              next_in=nxt, next_c=C, n_copies=n_copies, extra=extra if extra_c else None,
+                              extra_c=extra_c, extra_per_copy=case == "extra_per_copy",
+                              blend_x0=blend[0] if blend else None, blend_mask=blend[1] if blend else None,
+                              blend_noise=blend[2] if blend else None))
     torch.cuda.synchronize()
-    e = eps[:B] + 7.5 * (eps[B:] - eps[:B])
-    x0 = (lat_in - math.sqrt(1 - a_t) * e) / math.sqrt(a_t)
-    ref = math.sqrt(a_p) * x0 + math.sqrt(1 - a_p - sigma ** 2) * e + sigma * noise
-    assert (lat - ref).abs().max().item() < 1e-4
+    ref, bound = ref_cfg_ddim(eps_view, lat_in, noise, row, gscale, do_cfg, B, blend)
+    assert _within(lat, ref, bound), (case, ((lat.double() - ref).abs() / bound).max().item())
     assert step.item() == 2
-    for cpy in range(2):
-        blk = nxt[cpy * B:(cpy + 1) * B].float()
-        assert torch.equal(blk[..., :4], lat.to(BF16).float())
-        assert torch.equal(blk[..., 4:9], extra.to(BF16).float())
-        assert (blk[..., 9:] == 0).all()
+    for cpy in range(n_copies):
+        blk = nxt[cpy * B:(cpy + 1) * B]
+        assert torch.equal(blk[..., :4], lat.to(BF16)), (case, cpy)
+        if extra_c:
+            ex = extra[cpy * B:(cpy + 1) * B] if case == "extra_per_copy" else extra
+            assert torch.equal(blk[..., 4:9], ex.to(BF16)), cpy
+            assert (blk[..., 9:] == 0).all()
+        else:
+            assert blk[..., 4:].isnan().all()  # only the 4 latent channels are refreshed
+
+
+def test_unipc_step_kernel_matches_the_row_formula_and_replays_bit_identically(ops):
+    """pp_unipc_step against the fp64 row formula to an fp32 round-off bound, per element, for the corrector on and off,
+    CFG on and off, the three eps layouts and 1-3 copies of the net input; eager, program and graph runs
+    bit-identical; m2 <- m1 exactly, and next_in the bf16 rounding of the stored latents"""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    B, hw, C = 2, 37 * 13, 16
+    ucoef = torch.randn(3, 12, device=_dev(), generator=g)
+    coef = torch.full((3, 8), float("nan"), device=_dev())
+    coef[:, 5] = torch.tensor([7.5, 3.0, 1.5])
+    for use_c in (0.0, 1.0):
+        ucoef[1, 2] = use_c
+        for do_cfg in (False, True):
+            for n_copies in (1, 2, 3):
+                for eps_kind in ("fp32_vec", "fp32_strided", "bf16_strided"):
+                    nb = 2 * B if do_cfg else B
+                    eps, eps_fp32, eps_ld, eps_view = _eps_input(eps_kind, nb, hw, g)
+                    state0 = [torch.randn(B, hw, 4, device=_dev(), generator=g) for _ in range(4)]
+                    outs = []
+                    for mode in ("eager", "program", "graph"):
+                        lat, last, m1, m2 = (t.clone() for t in state0)
+                        nxt = torch.full((n_copies * B, hw, C), float("nan"), dtype=BF16, device=_dev())
+                        idx = torch.tensor([1], dtype=torch.int32, device=_dev())
+                        d = ops.unipc_desc(eps=eps, eps_fp32=eps_fp32, eps_ld=eps_ld, latents=lat, last_sample=last,
+                                           m1=m1, m2=m2, coef=coef, ucoef=ucoef, step_idx=idx,
+                                           advance_step=mode != "eager", do_cfg=do_cfg, batch=B, hw=hw, next_in=nxt,
+                                           next_c=C, n_copies=n_copies)
+                        if mode == "eager":
+                            ops.run(d)
+                        else:
+                            p = ops.Program()
+                            p.add(d)
+                            if mode == "graph":
+                                p.build_graph()
+                                p.launch()
+                            else:
+                                p.run()
+                        torch.cuda.synchronize()
+                        assert int(idx) == (1 if mode == "eager" else 2)
+                        outs.append((lat, last, m1, m2, nxt))
+                    tag = (use_c, do_cfg, n_copies, eps_kind)
+                    xn, xc, mt, bxn, bxc, bmt = ref_unipc(eps_view, *state0, ucoef[1], float(coef[1, 5]), do_cfg, B)
+                    lat, last, m1, m2, nxt = outs[0]
+                    assert _within(lat, xn, bxn), tag
+                    assert _within(last, xc, bxc), tag
+                    assert _within(m1, mt, bmt), tag
+                    assert torch.equal(m2, state0[2]), tag
+                    if not use_c:
+                        assert torch.equal(last, state0[0]), tag  # x_c = x: the stored sample is x itself
+                    for c in range(n_copies):
+                        assert torch.equal(nxt[c * B:(c + 1) * B, :, :4], lat.to(BF16)), tag
+                    assert nxt[..., 4:].isnan().all(), tag
+                    for o in outs[1:]:  # bit for bit (next_in keeps its NaN channels)
+                        assert all(torch.equal(a.view(torch.int16), b.view(torch.int16)) for a, b in zip(o, outs[0])), tag
 
 
 def test_program_and_graph(ops):

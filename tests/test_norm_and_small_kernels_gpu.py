@@ -36,10 +36,6 @@ SMS = 132
 COVERED_ELSEWHERE = {
     "gemm": "test_kernel_variants_gpu.py (variant matrix and GEMM census)",
     "attn": "test_kernel_variants_gpu.py (variant matrix and attention census)",
-    "cfg_ddim": "test_kernels_gpu.py::test_cfg_ddim and test_pipelines_gpu.py",
-    "unipc": "test_pipelines_gpu.py",
-    "solver": "test_solver_schedulers_gpu.py",
-    "plms": "test_pndm_gpu.py",
     "pool_broadcast": "test_side_net_modes_gpu.py",
     "window_copy": "test_vae_tiling_gpu.py",
     "tile_blend": "test_vae_tiling_gpu.py",
@@ -600,7 +596,8 @@ def census(ops):
     print(f"\n[op census] programs: denoisers {[s[0] for s in DENOISER_SHAPES]} under "
           f"{[s[0] for s in ENGINE_SWITCHES]}, VAE encode / decode 512x512, VAE tiled decode 80x80, text encoder")
     for kind in sorted(c.records):
-        where = "checked here" if kind in CHECKED_HERE else f"covered by {COVERED_ELSEWHERE.get(kind, '?')}"
+        where = "checked here" if kind in CHECKED_HERE else \
+            f"covered by {COVERED_ELSEWHERE.get(kind, 'test_program_replay_gpu.py')}"
         print(f"[op census]   {kind}: {c.records[kind]} records, {len(c.sigs.get(kind, {}))} signatures ({where})")
     return c
 
@@ -1095,8 +1092,10 @@ def test_time_embed(ops):
 @pytest.mark.gpu
 def test_census_op_kinds_are_all_covered(census):
     """every op kind the programs record is checked here or names the file that checks it; a new kind fails"""
+    from test_program_replay_gpu import REPLAY_EVALUATED  # the step kernels, on the programs' own activations
+
     recorded = set(census.records)
-    unknown = recorded - set(CHECKED_HERE) - set(COVERED_ELSEWHERE)
+    unknown = recorded - set(CHECKED_HERE) - set(COVERED_ELSEWHERE) - set(REPLAY_EVALUATED)
     assert not unknown, f"op kinds recorded by the programs but checked nowhere: {sorted(unknown)}"
     assert {"gn", "layer_norm", "add", "time_embed", "softmax_rows", "embed_gather", "causal_attention_small",
             "window_copy", "tile_blend", "memset"} <= recorded, sorted(recorded)

@@ -87,6 +87,8 @@ def test_solver_step_kernel_matches_the_row_formula_and_replays_bit_identically(
                     for c in range(n_copies):
                         blk = nxt[c * B:(c + 1) * B]
                         assert (blk[..., :4].double() - ni).abs().max() <= 8e-3 * max(1.0, float(ni.abs().max()))
+                        # bit for bit: bf16 of the fp32 product r6 * x_next of the stored x_next
+                        assert torch.equal(blk[..., :4], (scoef[1, 6] * lat).to(torch.bfloat16))
                         assert (blk[..., 4:] == 0).all()
                     for lat2, m12, nxt2 in outs[1:]:
                         assert torch.equal(lat2, lat) and torch.equal(m12, m1) and torch.equal(nxt2, nxt)
