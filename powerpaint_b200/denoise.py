@@ -178,6 +178,15 @@ class FusedDenoiser:
         st["bytes"] = pool.bytes
         return st
 
+    def record_slots(self, S: int, h: int, w: int, sched: str = "ddim", ctx_len: int = 77) -> "SlottedPlan":
+        """A step program with S independent slots (`SlottedPlan`); one pipeline mode, one latent size, classifier-free
+        guidance always on. Records nothing into the plan cache of `run`."""
+        if self.mode == "controlnet" and len(self.sides) != 1:
+            raise NotImplementedError("slotted plans take one ControlNet")
+        if any(getattr(s.config, "global_pool_conditions", False) for s in self.sides):
+            raise NotImplementedError("slotted plans take no globally pooled side net")
+        return SlottedPlan(self, S, h, w, sched, ctx_len)
+
     @property
     def launches_per_step(self) -> int:
         return max((s["program"].num_launches for s in self._cache.values()), default=0)
@@ -340,3 +349,195 @@ class FusedDenoiser:
         cur.wait_stream(self._stream)
         out.record_stream(cur)
         return out
+
+
+# A slot's table row that leaves its latents where they are: x_{t-1} = x_t, no history written. An idle slot replays
+# these rows, so its rows of the net input stay finite while other slots step.
+_HOLD = {"coef": [1.0, 0.0, 1.0, 0.0, 0.0, 1.0, 0.0, 0.0],
+         "ucoef": [0.0] * 7 + [1.0] + [0.0] * 4,          # use_c = 0, x_next = x
+         "scoef": [0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, 1.0],  # x_next = x, input scale 1
+         "pcoef": [1.0, 0.0, 0.0, 0.0, 0.0, 0.0, -1.0, 0.0]}  # x_next = x, no ring slot, no saved sample
+_SCHED_TABLE = {"ddim": None, "unipc": "ucoef", "solver": "scoef", "plms": "pcoef"}
+
+
+def _upload(dst: torch.Tensor, src: torch.Tensor) -> None:
+    """dst <- src without a host synchronisation: a host tensor is staged in pinned memory and copied asynchronously
+    (the pinned block is not reused before the copy has run)"""
+    if src.device.type == "cpu":
+        src = src.to(torch.float32).contiguous().pin_memory()
+        dst.copy_(src, non_blocking=True)
+    else:
+        dst.copy_(src)
+
+
+class SlottedPlan:
+    """One step program over S slots, each an independent request with its own step count, guidance scale, inputs and
+    side-net scale. Slot s owns the UNet rows 2s (unconditional) and 2s + 1 (conditional): the CFG pair of a slot is
+    contiguous, so every step kernel runs unchanged on one slot (batch 1, two copies of the next input).
+
+    Per slot the device holds a timestep table, an 8-float coefficient table (guidance in column 5), a side-net
+    scale x keep table, a step counter and the scheduler state. Each replay records, besides the shared nets, one time
+    embedding per slot, one step launch per slot (advancing that slot's counter) and, for a side net, one zero-conv
+    launch per slot and residual. `admit` loads a request's loop inputs (what the pipeline hands `FusedDenoiser.run`)
+    into a slot, `hold` parks a slot on rows that keep its latents fixed, `replay(k)` runs k steps of every slot."""
+
+    def __init__(self, fd: FusedDenoiser, S: int, h: int, w: int, sched: str, ctx_len: int):
+        if S < 1:
+            raise ValueError("a slotted plan needs at least one slot")
+        if sched not in _SCHED_TABLE:
+            raise ValueError(f"scheduler kind {sched!r}: one of {sorted(_SCHED_TABLE)}")
+        self.fd, self.S, self.h, self.w, self.sched, self.ctx_len = fd, S, h, w, sched, ctx_len
+        dev = fd.unet.device
+        hw, nb = h * w, 2 * S
+        f32 = dict(dtype=torch.float32, device=dev)
+        ue: NetEngine = fd.unet.engine()
+        self.program, self.ctx_program = ops.Program(), ops.Program()
+        self.x_in = torch.zeros(nb, hw, X_IN_C, dtype=torch.bfloat16, device=dev)
+        self.timesteps = torch.zeros(S, MAX_STEPS, **f32)
+        self.step_idx = torch.zeros(S, dtype=torch.int32, device=dev)
+        self.coef = torch.zeros(S, MAX_STEPS, 8, **f32)
+        self.side_scale = torch.zeros(S, MAX_STEPS, 1, **f32)
+        self.latents = torch.zeros(S, hw, 4, **f32)
+        self.pool = pool = Pool(dev)
+        steps = [(self.timesteps[s], self.step_idx[s:s + 1]) for s in range(S)]
+        common = dict(pool=pool, program=self.program, ctx_program=self.ctx_program, steps=steps)
+        down_s, mid_s, up_s = ue._state_shapes(nb, h, w)
+        nd = len(down_s)
+        shapes = {"v1": [], "brushnet": down_s + [mid_s] + up_s, "controlnet": down_s + [mid_s]}[fd.mode]
+        res = [pool.tensor(nb, hh * ww, c, zero=True) for (c, hh, ww) in shapes]
+        self.side_plan = None
+        if fd.side is not None:
+            side = SideOutputs(scale=(self.side_scale[0, :, 0], self.step_idx[:1], 1),
+                               targets=[b.reshape(-1, b.shape[-1]) for b in res],
+                               slot_scales=[(self.side_scale[s], self.step_idx[s:s + 1], 1) for s in range(S)])
+            self.side_plan = fd.side.engine()._build_plan(nb, h, w, ctx_len, x_in=self.x_in, side=side, **common)
+        self.uplan = ue._build_plan(nb, h, w, ctx_len, x_in=self.x_in, **common,
+                                    adds=(res[:nd], res[nd], res[nd + 1:]) if fd.mode == "brushnet" else None,
+                                    cn=(res[:nd], res[nd]) if fd.mode == "controlnet" else None)
+        self.state = {}  # scheduler state, one entry per slot per tensor
+        table = _SCHED_TABLE[sched]
+        if table is not None:
+            self.state[table] = torch.zeros(S, MAX_STEPS, len(_HOLD[table]), **f32)
+        if sched == "unipc":
+            for k in ("last_sample", "m1", "m2"):
+                self.state[k] = torch.zeros(S, hw, 4, **f32)
+        elif sched == "solver":
+            self.state["m1"] = torch.zeros(S, hw, 4, **f32)
+        elif sched == "plms":
+            self.state["cur_sample"] = torch.zeros(S, hw, 4, **f32)
+            # one ring per slot: the kernel's ring stride is batch x hw, so slots cannot share one [RING, S, hw, 4] ring
+            self.state["ets"] = [torch.zeros(PLMS_RING, 1, hw, 4, **f32) for _ in range(S)]
+        eps = self.uplan.outputs["eps"]
+        for s in range(S):
+            slot = dict(eps=eps[2 * s:2 * s + 2], eps_fp32=True, eps_ld=4, latents=self.latents[s:s + 1],
+                        coef=self.coef[s], step_idx=self.step_idx[s:s + 1], advance_step=True, do_cfg=True, batch=1,
+                        hw=hw, next_in=self.x_in[2 * s:2 * s + 2], next_c=X_IN_C, n_copies=2)
+            st = {k: v[s] if k in _HOLD or isinstance(v, list) else v[s:s + 1] for k, v in self.state.items()}
+            if sched == "unipc":
+                self.program.add(ops.unipc_desc(**slot, last_sample=st["last_sample"], m1=st["m1"], m2=st["m2"],
+                                                ucoef=st["ucoef"]))
+            elif sched == "solver":
+                self.program.add(ops.solver_desc(**slot, m1=st["m1"], scoef=st["scoef"]))
+            elif sched == "plms":
+                self.program.add(ops.plms_desc(**slot, cur_sample=st["cur_sample"], ets=st["ets"], pcoef=st["pcoef"]))
+            else:
+                self.program.add(ops.cfg_ddim_desc(**slot, noise=None, guidance_scale=0.0, guidance_from_coef=True))
+        self.bytes = pool.bytes
+        self.graph = False
+        # the hold rows of every table, on the device: parking a slot is a device-to-device copy
+        self._hold = {name: torch.tensor(_HOLD[name], **f32).expand(MAX_STEPS, len(_HOLD[name])).contiguous()
+                      for name in ("coef", table) if name is not None}
+        for s in range(S):
+            self.hold(s)
+
+    @property
+    def launches_per_step(self) -> int:
+        return self.program.num_launches
+
+    def hold(self, s: int) -> None:
+        """park slot s: latents zero, every table row a hold row, counter zero (its other input channels keep their
+        last, finite values)"""
+        self.latents[s].zero_()
+        self.x_in[2 * s:2 * s + 2, :, :4].zero_()
+        self.timesteps[s].zero_()
+        self.side_scale[s].zero_()
+        for name in ("coef", _SCHED_TABLE[self.sched]):
+            if name is not None:
+                t = self.coef if name == "coef" else self.state[name]
+                t[s].copy_(self._hold[name])
+        self.reset_counter(s)
+
+    def reset_counter(self, s: int) -> None:
+        self.step_idx[s:s + 1].zero_()
+
+    def admit(self, s: int, *, latents, prompt_embeds, timesteps, coef, guidance_scale, extra=None,
+              side_prompt_embeds=None, control_image=None, side_scale=1.0, side_keep=None, noise_fn=None, ucoef=None,
+              scoef=None, pcoef=None, blend=None, callback=None, guess_mode=False) -> int:
+        """load one request's loop inputs (the keywords the pipelines pass `FusedDenoiser.run`, for one image under
+        classifier-free guidance) into slot s and re-run the per-prompt programs; returns the request's step count"""
+        h, w, dev = self.h, self.w, self.x_in.device
+        if noise_fn is not None or blend is not None or callback is not None or guess_mode:
+            raise NotImplementedError("slots take no per-step noise, 4-channel blend, callback or guess mode")
+        if tuple(latents.shape) != (1, 4, h, w) or prompt_embeds.shape[0] != 2:
+            raise ValueError(f"a slot takes one {h}x{w} latent and its [negative; positive] prompt rows")
+        given = {"ucoef": ucoef, "scoef": scoef, "pcoef": pcoef}
+        table = _SCHED_TABLE[self.sched]
+        if any(v is not None for k, v in given.items() if k != table) or (table and given[table] is None):
+            raise ValueError(f"the plan was recorded for scheduler kind {self.sched!r}")
+        n = len(timesteps)
+        if not 1 <= n <= MAX_STEPS:
+            raise ValueError(f"1 to {MAX_STEPS} steps")
+        rows = slice(2 * s, 2 * s + 2)
+        in_scale = 1.0
+        if table is not None:
+            tab = given[table].to(torch.float32)
+            if len(tab) != n:
+                raise ValueError(f"{table} needs one row per step")
+            _upload(self.state[table][s, :n], tab)
+            if table == "scoef":
+                in_scale = float(tab[0, 7])
+            for k, v in self.state.items():
+                if k != table:
+                    v[s].zero_()
+        lat = ops.nhwc_fp32_from_nchw(latents.to(dev, torch.float32))
+        self.latents[s:s + 1].copy_(lat)
+        self.x_in[rows, :, :4] = (lat * in_scale if in_scale != 1.0 else lat).to(torch.bfloat16)
+        if extra is not None:
+            self.x_in[rows, :, 4:9] = ops.nhwc_fp32_from_nchw(extra.to(dev, torch.float32)).to(torch.bfloat16)
+        else:
+            self.x_in[rows, :, 4:9] = 0
+        _upload(self.timesteps[s, :n], torch.as_tensor([float(t) for t in timesteps], dtype=torch.float32))
+        cf = coef.clone().float()
+        cf[:, COEF_GUIDANCE] = float(guidance_scale)
+        _upload(self.coef[s, :n], cf)
+        keep = torch.ones(n) if side_keep is None else torch.tensor([float(v) for v in side_keep])
+        if len(keep) != n:
+            raise ValueError("side_keep needs one entry per step")
+        _upload(self.side_scale[s, :n, 0], float(side_scale) * keep)
+        self.uplan.inputs["ctx"][rows].copy_(prompt_embeds.to(dev, torch.bfloat16))
+        if self.side_plan is not None:
+            if side_prompt_embeds is None:
+                raise ValueError("side_prompt_embeds required")
+            self.side_plan.inputs["ctx"][rows].copy_(side_prompt_embeds[-2:].to(dev, torch.bfloat16))
+            if self.fd.mode == "controlnet":
+                img = control_image[0] if isinstance(control_image, (list, tuple)) else control_image
+                if img is None or img.shape[0] != 2:
+                    raise ValueError("control_image: one image per CFG half")
+                ci = self.side_plan.inputs["cond_in"]
+                ci[rows].copy_(ops.nchw_to_nhwc(img.to(dev).float().contiguous(), ci.shape[-1]).view_as(ci[rows]))
+                self.side_plan.cond_program.run()
+        self.ctx_program.run()
+        self.reset_counter(s)
+        return n
+
+    def replay(self, k: int) -> None:
+        """k steps of every slot: the captured graph, captured on first use"""
+        if not self.graph:
+            self.program.build_graph()
+            self.graph = True
+        for _ in range(k):
+            self.program.launch()
+
+    def slot_latents(self, s: int) -> torch.Tensor:
+        """slot s's latents [1, 4, h, w] fp32 (a copy)"""
+        return ops.nchw_from_nhwc_fp32(self.latents[s:s + 1], self.h, self.w).clone()

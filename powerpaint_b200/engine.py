@@ -197,6 +197,9 @@ class SideOutputs:
     global_pool: bool = False  # the scaled output is replaced by its spatial mean, broadcast to full size, before prev_k
     targets: Optional[List[torch.Tensor]] = None  # buffers to write into (None: fresh ones that are never recycled)
     prev: Optional[List[torch.Tensor]] = None  # residuals of the previous net of a Multi-ControlNet to add (None: none)
+    # slotted plans: one (tensor, step index, stride) per slot, replacing `scale`. Each residual is then written by one
+    # launch per slot over that slot's equal share of the rows, reading the slot's own scale table and step counter
+    slot_scales: Optional[List[Tuple[torch.Tensor, torch.Tensor, int]]] = None
 
 
 class Recorder:
@@ -659,7 +662,8 @@ class NetEngine(Recorder):
         of one fused step pass the same three, so they share one program and one activation pool.
         `x_in`: a [nb, h*w, C] buffer whose first channels are this net's input; extra channels meet zero weights
         (default: a fresh input buffer). `steps` = (timesteps table, step index): the time embedding reads the
-        timestep of the device-side step counter (default: per-sample timesteps, `plan.inputs["timesteps"]`).
+        timestep of the device-side step counter (default: per-sample timesteps, `plan.inputs["timesteps"]`); a list
+        of such pairs, one per slot, gives each slot's equal share of the rows its own table and counter.
         UNet: `adds` = (down, mid, up) BrushNet adds / `cn` = (down, mid) ControlNet residuals to read.
         Side nets: `side` says where their zero-convs write (`_zero_convs`)."""
         cfg = self.cfg
@@ -693,7 +697,12 @@ class NetEngine(Recorder):
         ctx = pool.tensor(nb, ctx_len, cfg.cross_attention_dim, zero=True)
         plan.inputs["x_in"] = x_in
         plan.inputs["ctx"] = ctx
-        if steps is not None:
+        slot_steps = steps if isinstance(steps, list) else None
+        if slot_steps is not None:
+            if nb % len(slot_steps):
+                raise ValueError("the rows must split evenly over the slots")
+            plan.inputs["slot_steps"] = slot_steps
+        elif steps is not None:
             plan.inputs["timesteps"], plan.inputs["step_idx"] = steps
         else:
             plan.inputs["timesteps"] = torch.zeros(nb, dtype=torch.float32, device=self.device)
@@ -707,7 +716,12 @@ class NetEngine(Recorder):
 
         # ---------------- time embedding (unet_2d_condition.py:1155-1156) + stacked time_emb_proj
         tsin = plan.pool.buf(nb, C0)
-        prog.add_time_embed(plan.inputs["timesteps"], plan.inputs.get("step_idx"), tsin, nb, C0)
+        if slot_steps is not None:
+            r = nb // len(slot_steps)
+            for s, (ts, si) in enumerate(slot_steps):
+                prog.add_time_embed(ts, si, tsin[s * r:(s + 1) * r], r, C0)
+        else:
+            prog.add_time_embed(plan.inputs["timesteps"], plan.inputs.get("step_idx"), tsin, nb, C0)
         e1 = self._linear(plan, prog, tsin, nb, "time_embedding.linear_1", temb_c,
                           bias=self.vec("time_embedding.linear_1.bias"), act=N.PP_ACT_SILU)
         # resnets consume silu(emb); emb itself is not used elsewhere on the SD-1.5 path
@@ -888,7 +902,15 @@ class NetEngine(Recorder):
             prev = side.prev[k] if side.prev is not None else None
             kw = dict(bias=self.vec(wname + ".bias"), alpha=side.alphas[k] if side.alphas else 1.0,
                       alpha_dev=sdev, alpha_step=sstep, alpha_stride=sstride)
-            if side.global_pool:
+            if side.slot_scales is not None:
+                if side.global_pool or prev is not None:
+                    raise ValueError("slotted zero-convs take neither global pooling nor a previous net's residuals")
+                r = M // len(side.slot_scales)
+                a, o = st.reshape(M, c), out.view(M, c)
+                for s, (sd, ss, sr) in enumerate(side.slot_scales):
+                    self._linear(plan, prog, a[s * r:(s + 1) * r], r, wname, c, out=o[s * r:(s + 1) * r],
+                                 **dict(kw, alpha_dev=sd, alpha_step=ss, alpha_stride=sr))
+            elif side.global_pool:
                 z = plan.pool.buf(M, c)
                 self._linear(plan, prog, st, M, wname, c, out=z, **kw)
                 shape = (nb, M // nb, c)

@@ -8,7 +8,7 @@ Restated from the reference: `prepare_mask_and_masked_image`
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Optional, Union
+from typing import Callable, List, Optional, Union
 
 import numpy as np
 import PIL.Image
@@ -19,6 +19,31 @@ import torch
 class StableDiffusionPipelineOutput:
     images: Union[List[PIL.Image.Image], np.ndarray, torch.Tensor]
     nsfw_content_detected: Optional[List[bool]]
+
+
+@dataclass
+class LoopInputs:
+    """What a pipeline's `prepare_loop` hands the fused denoising loop for one call: `run`, the keywords of
+    `FusedDenoiser.run`; `finish`, None or what the scheduler does after the loop; and the call's output options."""
+    run: dict
+    finish: Optional[Callable[[], None]]
+    output_type: Optional[str]
+    return_dict: bool
+
+
+def run_loop(pipe, loop: LoopInputs):
+    """the tail of every pipeline's `__call__`: the fused loop over `loop.run`, the scheduler's `finish`, the decode"""
+    return loop_output(pipe, loop, pipe.denoiser().run(**loop.run))
+
+
+def loop_output(pipe, loop: LoopInputs, latents: torch.Tensor):
+    """what `__call__` returns for the final latents of `loop`, after the scheduler's `finish`"""
+    if loop.finish is not None:
+        loop.finish()
+    image = latents if loop.output_type == "latent" else decode_latents(pipe.vae, latents, loop.output_type)
+    if not loop.return_dict:
+        return (image, None)
+    return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=None)
 
 
 def randn_tensor(shape, generator=None, device=None, dtype=None):

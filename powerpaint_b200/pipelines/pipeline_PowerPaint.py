@@ -19,8 +19,8 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models import AutoencoderKL, BrushNetModel, ControlNetModel, UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, callback_fires, decode_latents, encode_text,
-                     prepare_mask_and_masked_image, randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
+from .common import (LoopInputs, callback_fires, decode_latents, encode_text, prepare_mask_and_masked_image, run_loop,
+                     randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
 
 # the components stored as diffusers model directories, by their name in model_index.json
 _MODEL_COMPONENTS = {"unet": UNet2DConditionModel, "brushnet": BrushNetModel, "controlnet": ControlNetModel,
@@ -359,7 +359,12 @@ class StableDiffusionInpaintPipeline:
 
     # ------------------------------------------------------------------ __call__ (:722-1071)
     @torch.no_grad()
-    def __call__(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None, image=None,
+    def __call__(self, *args, **kwargs):
+        """`prepare_loop`'s arguments: prepares the call, runs the fused denoising loop and decodes"""
+        return run_loop(self, self.prepare_loop(*args, **kwargs))
+
+    @torch.no_grad()
+    def prepare_loop(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None, image=None,
                  mask=None, height: Optional[int] = None, width: Optional[int] = None, strength: float = 1.0,
                  tradoff: float = 1.0, tradoff_nag: float = 1.0, num_inference_steps: int = 50,
                  guidance_scale: float = 7.5, negative_promptA: Optional[Union[str, List[str]]] = None,
@@ -467,13 +472,8 @@ class StableDiffusionInpaintPipeline:
         # `scoef` / `pcoef` are passed only when such a scheduler is set: a denoiser whose `run` predates those kinds
         # keeps serving DDIM and UniPC unchanged
         opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
-        latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, timesteps=timesteps, coef=coef,
-                                      guidance_scale=guidance_scale,
-                                      extra=torch.cat([mask, masked_image_latents], dim=1) if num_channels_unet == 9
-                                      else None, noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb, **opt)
-        if finish is not None:
-            finish()
-        image = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
-        if not return_dict:
-            return (image, None)
-        return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=None)
+        run = dict(latents=latents, prompt_embeds=prompt_embeds, timesteps=timesteps, coef=coef,
+                   guidance_scale=guidance_scale,
+                   extra=torch.cat([mask, masked_image_latents], dim=1) if num_channels_unet == 9 else None,
+                   noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb, **opt)
+        return LoopInputs(run, finish, output_type, return_dict)

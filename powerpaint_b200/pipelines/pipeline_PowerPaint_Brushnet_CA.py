@@ -20,8 +20,8 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import BrushNetModel, UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, callback_fires, check_control_guidance, check_image,
-                     check_prompt_arguments, decode_latents, encode_text, preprocess_image, randn_tensor,
+from .common import (LoopInputs, callback_fires, check_control_guidance, check_image, check_prompt_arguments,
+                     encode_text, preprocess_image, randn_tensor,
                      solver_loop_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
@@ -177,7 +177,7 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
 
     # ------------------------------------------------------------------ __call__ (:1024-1497)
     @torch.no_grad()
-    def __call__(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None,
+    def prepare_loop(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None,
                  promptU: Union[str, List[str]] = None, tradoff: float = 1.0, tradoff_nag: float = 1.0, image=None,
                  mask=None, height: Optional[int] = None, width: Optional[int] = None, num_inference_steps: int = 50,
                  timesteps: List[int] = None, guidance_scale: float = 7.5,
@@ -328,14 +328,8 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
         if guess_mode:
             opt["guess_mode"] = True
-        latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds,
-                                      timesteps=ts, coef=coef, guidance_scale=guidance_scale,
-                                      extra=conditioning_latents, side_scale=float(brushnet_conditioning_scale),
-                                      side_keep=keep, ucoef=ucoef,
-                                      noise_fn=noise_fn, callback=cb, **opt)
-        if finish is not None:
-            finish()
-        image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
-        if not return_dict:
-            return (image_o, None)
-        return StableDiffusionPipelineOutput(images=image_o, nsfw_content_detected=None)
+        run = dict(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds, timesteps=ts,
+                   coef=coef, guidance_scale=guidance_scale, extra=conditioning_latents,
+                   side_scale=float(brushnet_conditioning_scale), side_keep=keep, ucoef=ucoef, noise_fn=noise_fn,
+                   callback=cb, **opt)
+        return LoopInputs(run, finish, output_type, return_dict)

@@ -19,8 +19,8 @@ import torch
 
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import ControlNetModel, MultiControlNetModel, UNet2DConditionModel
-from .common import (StableDiffusionPipelineOutput, callback_fires, check_control_guidance, check_image,
-                     check_prompt_arguments, decode_latents, prepare_mask_and_masked_image, preprocess_image,
+from .common import (LoopInputs, callback_fires, check_control_guidance, check_image, check_prompt_arguments,
+                     prepare_mask_and_masked_image, preprocess_image,
                      randn_tensor, solver_loop_inputs, uint8_device_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
@@ -121,7 +121,7 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
         return image
 
     @torch.no_grad()
-    def __call__(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None, image=None,
+    def prepare_loop(self, promptA: Union[str, List[str]] = None, promptB: Union[str, List[str]] = None, image=None,
                  mask=None, control_image=None, height: Optional[int] = None, width: Optional[int] = None,
                  strength: float = 1.0, tradoff: float = 1.0, tradoff_nag: float = 1.0, num_inference_steps: int = 50,
                  guidance_scale: float = 7.5, negative_promptA: Optional[Union[str, List[str]]] = None,
@@ -239,13 +239,7 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             side["scoef"] = scoef
         if pcoef is not None:
             side["pcoef"] = pcoef
-        latents = self.denoiser().run(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds,
-                                      timesteps=timesteps, coef=coef, guidance_scale=guidance_scale,
-                                      extra=torch.cat([mask, masked_image_latents], dim=1),
-                                      noise_fn=noise_fn, ucoef=ucoef, callback=cb, **side)
-        if finish is not None:
-            finish()
-        image_o = latents if output_type == "latent" else decode_latents(self.vae, latents, output_type)
-        if not return_dict:
-            return (image_o, None)
-        return StableDiffusionPipelineOutput(images=image_o, nsfw_content_detected=None)
+        run = dict(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds, timesteps=timesteps,
+                   coef=coef, guidance_scale=guidance_scale, extra=torch.cat([mask, masked_image_latents], dim=1),
+                   noise_fn=noise_fn, ucoef=ucoef, callback=cb, **side)
+        return LoopInputs(run, finish, output_type, return_dict)

@@ -207,6 +207,18 @@ def run_cases(out_dir, switch, census_only):
         torch.cuda.empty_cache()
     if census_only:
         return written
+    # slotted step programs (serving.RequestBatcher): 4 slots at 64 x 64 latents, one per mode and scheduler kind
+    from powerpaint_b200.denoise import FusedDenoiser
+
+    for name, d, sched in (("slotted_v1_ddim", FusedDenoiser(m["u9"]), "ddim"),
+                           ("slotted_v1_plms", FusedDenoiser(m["u9"]), "plms"),
+                           ("slotted_v1_solver", FusedDenoiser(m["u9"]), "solver"),
+                           ("slotted_brushnet_unipc", FusedDenoiser(m["u4"], m["bn"], "brushnet"), "unipc"),
+                           ("slotted_controlnet_ddim", FusedDenoiser(m["u9"], m["cn"], "controlnet"), "ddim")):
+        sp = d.record_slots(4, 64, 64, sched)
+        emit(name, [f"bytes={sp.bytes}"])
+        del d, sp
+        torch.cuda.empty_cache()
     g = torch.Generator(device=dev).manual_seed(0)
     B, h, w = 2, 64, 64
     t = torch.tensor(500.0)
