@@ -334,6 +334,26 @@ pp_status pp_embed_gather(const int32_t* idx, const float* base, const float* ex
 pp_status pp_causal_attention_small(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, int32_t d,
                                     float scale, pp_stream stream);
 
+/* ------------------------------------------------------------------ device-drawn step noise */
+/* One draw of torch's CUDA randn: the noise a stochastic step adds is, element for element,
+   `torch.randn(shape, generator=g, device="cuda", dtype=torch.float32)` of a draw of N = rows * 4 * hw elements
+   (NCHW [rows, 4, h, w]), computed by the step kernel where it uses it. torch's launch policy fixes every element:
+     threads = 256 * min(ceil(N / 256), SMs * (maxThreadsPerSM / 256)),   q = li / threads
+     element li = lane q % 4 of the (q / 4)-th curand_normal4 of curand_init(seed, li % threads, offset)
+   and each draw advances the generator by offset_per_step = ((N - 1) / (threads * 4) + 1) * 4.
+   The draw of step s uses offset = offset0 + s * offset_per_step (s = *step_idx of the step descriptor), so a
+   replayed CUDA graph needs nothing from the host. Latent row b in [first_row, first_row + rows), pixel p and
+   channel c of the NHWC step tensors take element li = ((b - first_row) * 4 + c) * hw + p. The host reserves the
+   generator's stream (advances its offset past the loop's draws) when it fills the table. */
+typedef struct pp_randn_draw {
+    uint64_t seed;
+    uint64_t offset0;
+    uint64_t offset_per_step;
+    int64_t threads;      /* 256 * grid of torch's launch for this draw */
+    int32_t first_row;    /* latent rows [first_row, first_row + rows) of the step take this draw */
+    int32_t rows;         /* 0: the entry matches no row */
+} pp_randn_draw;
+
 /* ------------------------------------------------------------------ CFG + DDIM */
 typedef struct pp_cfg_ddim_desc {
     /* eps: model output for the 2*batch CFG-duplicated samples (unconditional half first),
@@ -370,6 +390,11 @@ typedef struct pp_cfg_ddim_desc {
     const float* blend_x0;
     const float* blend_mask;
     const float* blend_noise;
+    /* device-drawn variance noise (pp_randn_draw): n_draws entries, 8-byte aligned; a row no entry covers gets
+       zero noise. Exclusive with `noise`. Nothing is drawn when sigma (coef[row][4]) is exactly 0, so a table whose
+       rows all have sigma 0 gives the same bits as draws = NULL. NULL / 0 = none. */
+    const pp_randn_draw* draws;
+    int32_t n_draws;
 } pp_cfg_ddim_desc;
 pp_status pp_cfg_ddim_step(const pp_cfg_ddim_desc* d, pp_stream stream);
 
@@ -424,6 +449,10 @@ typedef struct pp_solver_desc {
     int32_t batch, hw;
     void* next_in;       /* bf16 NHWC [n_copies*batch, hw, next_c]: channels 0..3 refreshed */
     int32_t next_c, n_copies;
+    /* device-drawn noise, as pp_cfg_ddim_desc.draws: exclusive with `noise`; nothing is drawn when r[5] is
+       exactly 0. NULL / 0 = none. */
+    const pp_randn_draw* draws;
+    int32_t n_draws;
 } pp_solver_desc;
 pp_status pp_solver_step(const pp_solver_desc* d, pp_stream stream);
 

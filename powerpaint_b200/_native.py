@@ -25,6 +25,7 @@ vp = C.c_void_p
 i32 = C.c_int32
 i64 = C.c_int64
 f32 = C.c_float
+u64 = C.c_uint64
 
 
 class StatsGeom(C.Structure):
@@ -80,6 +81,12 @@ class GnDesc(C.Structure):
     ]
 
 
+class RandnDraw(C.Structure):
+    """pp_randn_draw: one draw of torch's CUDA randn, computed inside the step kernels"""
+    _fields_ = [("seed", u64), ("offset0", u64), ("offset_per_step", u64), ("threads", i64),
+                ("first_row", i32), ("rows", i32)]
+
+
 class CfgDdimDesc(C.Structure):
     _fields_ = [
         ("eps", vp), ("eps_fp32", i32), ("eps_ld", i32),
@@ -89,6 +96,7 @@ class CfgDdimDesc(C.Structure):
         ("next_in", vp), ("next_c", i32), ("n_copies", i32),
         ("extra", vp), ("extra_c", i32), ("guidance_from_coef", i32), ("extra_per_copy", i32),
         ("blend_x0", vp), ("blend_mask", vp), ("blend_noise", vp),
+        ("draws", vp), ("n_draws", i32),
     ]
 
 
@@ -109,6 +117,7 @@ class SolverDesc(C.Structure):
         ("coef", vp), ("scoef", vp), ("step_idx", vp), ("advance_step", i32), ("do_cfg", i32),
         ("batch", i32), ("hw", i32),
         ("next_in", vp), ("next_c", i32), ("n_copies", i32),
+        ("draws", vp), ("n_draws", i32),
     ]
 
 

@@ -1,9 +1,47 @@
 // HBM-bound glue kernels of the denoising step: fused CFG + DDIM update (+ next UNet input),
 // sinusoidal timestep embedding, nearest 2x upsample, residual add, NCHW<->NHWC conversion.
+#include <curand_kernel.h>  // header-only device API: Philox4x32-10 and the Box-Muller torch's CUDA randn compiles
+
 #include "common.cuh"
 #include "ops.h"
 
 namespace pp {
+
+// ------------------------------------------------------------------------------------
+// Element li of torch's CUDA randn for one draw (pp_randn_draw, include/powerpaint_b200.h), at the draw's Philox
+// offset `offset`. torch's grid-stride kernel (ATen/native/cuda/DistributionTemplates.h) gives thread t the elements
+// t + threads * q, the q-th one as lane q % 4 of its (q / 4)-th curand_normal4; a state initialised (q / 4) * 4
+// further along the counter makes that call its first.
+// ------------------------------------------------------------------------------------
+__device__ __forceinline__ float torch_randn_at(const pp_randn_draw& d, unsigned long long offset, int64_t li) {
+    const int64_t q = li / d.threads;
+    curandStatePhilox4_32_10_t st;
+    curand_init(d.seed, (unsigned long long)(li - q * d.threads), offset + (unsigned long long)(q >> 2) * 4ull, &st);
+    const float4 r = curand_normal4(&st);
+    const int lane = (int)(q & 3);
+    return lane == 0 ? r.x : lane == 1 ? r.y : lane == 2 ? r.z : r.w;
+}
+
+// The four channels of NHWC pixel i (row i / hw) of a step's noise, from the draw that covers the row (zero if none).
+__device__ __forceinline__ void randn_nhwc(const pp_randn_draw* __restrict__ draws, int n_draws, int step, int64_t i,
+                                           int hw, float nz[4]) {
+    const int64_t b = i / hw, p = i - b * hw;
+    for (int k = 0; k < n_draws; ++k) {
+        const pp_randn_draw d = draws[k];
+        if (b < d.first_row || b >= (int64_t)d.first_row + d.rows) continue;
+        const unsigned long long off = d.offset0 + (unsigned long long)step * d.offset_per_step;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) nz[c] = torch_randn_at(d, off, ((b - d.first_row) * 4 + c) * hw + p);
+        return;
+    }
+}
+
+static int draws_validate(const void* noise, const pp_randn_draw* draws, int32_t n_draws, const char* what) {
+    PP_REQUIRE(n_draws >= 0 && (draws == nullptr) == (n_draws == 0), "%s: draws and n_draws go together", what);
+    PP_REQUIRE(!(noise && draws), "%s: noise and draws are exclusive", what);
+    PP_REQUIRE((reinterpret_cast<uintptr_t>(draws) & 7) == 0, "%s: draws need 8-byte alignment", what);
+    return PP_OK;
+}
 
 // ------------------------------------------------------------------------------------
 // Fused classifier-free guidance + DDIMScheduler.step + next-input build.
@@ -60,6 +98,8 @@ __global__ void cfg_ddim_kernel(pp_cfg_ddim_desc d) {
         if (d.noise) {
             float4 n4 = *reinterpret_cast<const float4*>(d.noise + i * 4);
             nz[0] = n4.x; nz[1] = n4.y; nz[2] = n4.z; nz[3] = n4.w;
+        } else if (d.draws && sigma != 0.f) {
+            randn_nhwc(d.draws, d.n_draws, step, i, d.hw, nz);
         }
         float xp[4];
 #pragma unroll
@@ -125,6 +165,7 @@ int cfg_ddim_validate(const pp_cfg_ddim_desc& d) {
                "cfg_ddim: fp32 eps with eps_ld 4 needs 16-byte alignment");
     PP_REQUIRE((reinterpret_cast<uintptr_t>(d.blend_x0) & 15) == 0 && (reinterpret_cast<uintptr_t>(d.blend_noise) & 15) == 0,
                "cfg_ddim: blend_x0 / blend_noise need 16-byte alignment");
+    if (int rc = draws_validate(d.noise, d.draws, d.n_draws, "cfg_ddim")) return rc;
     if (d.next_in) {
         PP_REQUIRE(d.next_c >= 4 && d.n_copies >= 1, "cfg_ddim: next_in needs next_c >= 4, n_copies >= 1");
         PP_REQUIRE(d.extra_c == 0 || d.extra, "cfg_ddim: extra_c without extra");
@@ -244,7 +285,8 @@ int unipc_launch(const pp_unipc_desc& d, cudaStream_t s) {
 // Euler / Euler-ancestral + next-input refresh. All of them are linear in (x, eps, previous x0 prediction,
 // noise), so the host folds each step into one 8-float row (include/powerpaint_b200.h, pp_solver_desc).
 // One thread per pixel, 16-byte accesses. Algorithmic bytes per pixel (CFG, fp32 eps): eps 32 + latents 16 + 16 +
-// m1 16 + 16 + next input 2 x 8 = 112 B; + 16 B of noise for the SDE / ancestral variants.
+// m1 16 + 16 + next input 2 x 8 = 112 B; + 16 B of noise for the SDE / ancestral variants, or none when the
+// noise is drawn in the kernel (pp_randn_draw: four Philox4x32-10 evaluations and Box-Muller pairs per pixel).
 // ------------------------------------------------------------------------------------
 __global__ void solver_step_kernel(pp_solver_desc d) {
     pdl_wait();
@@ -278,7 +320,8 @@ __global__ void solver_step_kernel(pp_solver_desc d) {
         float4 n4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (d.noise) n4 = __ldg(reinterpret_cast<const float4*>(d.noise) + i);
         const float x[4] = {x4.x, x4.y, x4.z, x4.w}, m1[4] = {a4.x, a4.y, a4.z, a4.w};
-        const float nz[4] = {n4.x, n4.y, n4.z, n4.w};
+        float nz[4] = {n4.x, n4.y, n4.z, n4.w};
+        if (d.draws && r5 != 0.f) randn_nhwc(d.draws, d.n_draws, step, i, d.hw, nz);
         float mt[4], xn[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -306,6 +349,7 @@ int solver_validate(const pp_solver_desc& d) {
                "solver: latents / m1 / noise need 16-byte alignment");
     PP_REQUIRE(!(d.eps_fp32 && d.eps_ld == 4) || (reinterpret_cast<uintptr_t>(d.eps) & 15) == 0,
                "solver: fp32 eps with eps_ld 4 needs 16-byte alignment");
+    if (int rc = draws_validate(d.noise, d.draws, d.n_draws, "solver")) return rc;
     if (d.next_in)
         PP_REQUIRE(d.next_c >= 4 && d.next_c % 4 == 0 && d.n_copies >= 1 && (reinterpret_cast<uintptr_t>(d.next_in) & 7) == 0,
                    "solver: next_in needs next_c %% 4 == 0, n_copies >= 1 and 8-byte alignment");

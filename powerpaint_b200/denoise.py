@@ -82,18 +82,22 @@ class FusedDenoiser:
 
     # ------------------------------------------------------------------ plan
     def _get(self, B: int, h: int, w: int, do_cfg: bool, ctx_len: int, with_noise: bool,
-             extra_per_copy: bool, sched: str = "ddim", blend: bool = False, guess: bool = False) -> dict:
+             extra_per_copy: bool, sched: str = "ddim", blend: bool = False, guess: bool = False,
+             device_noise: bool = False) -> dict:
         pools = tuple(bool(getattr(s.config, "global_pool_conditions", False)) for s in self.sides)
         # the key carries the parameter generation of each model: `load_state_dict` / `.to()` invalidate it,
         # and the cached entry keeps its engines alive, so a recycled id() can never alias a stale program
-        key = (B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, len(self.sides), guess, pools,
-               self.unet.generation, tuple(s.generation for s in self.sides))
+        key = (B, h, w, do_cfg, ctx_len, with_noise, device_noise, extra_per_copy, sched, blend, len(self.sides), guess,
+               pools, self.unet.generation, tuple(s.generation for s in self.sides))
         for k in [k for k in self._cache if k[-2:] != key[-2:]]:  # (unet generation, side generations)
             del self._cache[k]  # plans recorded against replaced weights
         return lru_get(self._cache, key, self.MAX_PLANS, lambda: self._record(
-            B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools))
+            B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools, device_noise))
 
-    def _record(self, B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools) -> dict:
+    def _record(self, B, h, w, do_cfg, ctx_len, with_noise, extra_per_copy, sched, blend, guess, pools,
+                device_noise=False) -> dict:
+        """`with_noise`: the step reads host-drawn noise from st["noise"]; `device_noise`: the step kernel draws it
+        from the B-entry pp_randn_draw table st["draws"]"""
         K = len(self.sides)
         dev = self.unet.device
         nb = 2 * B if do_cfg else B
@@ -134,6 +138,8 @@ class FusedDenoiser:
         st["latents"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
         st["extra"] = torch.zeros(n_extra, h * w, 5, dtype=torch.float32, device=dev)
         st["noise"] = torch.zeros(B, h * w, 4, dtype=torch.float32, device=dev)
+        # one entry per latent row at most (a list of generators); the entries a call does not use match no row
+        st["draws"] = torch.zeros(B * ops.RANDN_DRAW_BYTES, dtype=torch.uint8, device=dev) if device_noise else None
         if sched == "unipc":
             # UniPCMultistepScheduler (the v2 app's scheduler, app.py:197): multistep state lives next to the latents
             for k in ("last_sample", "m1", "m2"):
@@ -150,7 +156,7 @@ class FusedDenoiser:
             prog.add(ops.solver_desc(eps=uplan.outputs["eps"], eps_fp32=True, eps_ld=4, latents=st["latents"],
                                      m1=st["m1"], coef=coef, scoef=st["scoef"], step_idx=step_idx, advance_step=True,
                                      do_cfg=do_cfg, batch=B, hw=h * w, noise=st["noise"] if with_noise else None,
-                                     next_in=x_in, next_c=X_IN_C, n_copies=2 if do_cfg else 1))
+                                     draws=st["draws"], next_in=x_in, next_c=X_IN_C, n_copies=2 if do_cfg else 1))
         else:
             if blend:  # 4-channel UNet: known region kept on the noised original after every step
                 st["blend_x0"] = torch.zeros(h * w, 4, dtype=torch.float32, device=dev)
@@ -170,7 +176,7 @@ class FusedDenoiser:
         elif sched == "ddim":
             prog.add(ops.cfg_ddim_desc(eps=uplan.outputs["eps"], eps_fp32=True, eps_ld=4, latents=st["latents"],
                                        coef=coef, step_idx=step_idx, advance_step=True,
-                                       noise=st["noise"] if with_noise else None, guidance_scale=0.0,
+                                       noise=st["noise"] if with_noise else None, draws=st["draws"], guidance_scale=0.0,
                                        guidance_from_coef=True, do_cfg=do_cfg, batch=B, hw=h * w, next_in=x_in,
                                        next_c=X_IN_C, n_copies=2 if do_cfg else 1, extra=None, extra_c=0,
                                        blend_x0=st.get("blend_x0"), blend_mask=st.get("blend_mask"),
@@ -209,7 +215,7 @@ class FusedDenoiser:
             noise_fn: Optional[Callable[[int], torch.Tensor]] = None, ucoef: Optional[torch.Tensor] = None,
             scoef: Optional[torch.Tensor] = None, pcoef: Optional[torch.Tensor] = None, blend: Optional[dict] = None,
             callback: Optional[Callable[[int, int, torch.Tensor], Optional[torch.Tensor]]] = None,
-            use_graph: bool = True, guess_mode: bool = False) -> torch.Tensor:
+            use_graph: bool = True, guess_mode: bool = False, randn_draws=None) -> torch.Tensor:
         """latents [B,4,h,w]; prompt_embeds [nb,77,768] for the UNet (negative half first when CFG);
         extra [B or nb,5,h,w] = constant channels (v1/controlnet: mask + masked-image latents;
         brushnet: conditioning latents + mask; nb rows = one set per CFG half); side_prompt_embeds
@@ -223,6 +229,9 @@ class FusedDenoiser:
         (a callback's replacement latents after step 0 only feed step 1's net input: that step restarts from the
         sample step 0 started at, as in diffusers); `blend` = dict(x0 [1,4,h,w], mask [1,1,h,w], noise [B,4,h,w],
         sqrt_alpha [n]) is the 4-channel-UNet blend (ref pipeline_PowerPaint.py:1025-1035).
+        `randn_draws` (exclusive with `noise_fn`): the noise of the stochastic steps drawn by the step kernels, rows of
+        pp_randn_draw fields (`pipelines.common.device_randn_draws`) covering the B latent rows; step i draws
+        at offset0 + i * offset_per_step, so the loop stays one CUDA graph.
         `callback(i, t, latents_nchw)` may return replacement
         latents. Returns the final latents [B,4,h,w] fp32.
         K ControlNets: `side_scale` a list of K floats, `side_keep` None or a list of K per-step lists,
@@ -259,14 +268,21 @@ class FusedDenoiser:
                 raise ValueError("ucoef, scoef and pcoef select different step kernels: pass one")
             sched = "unipc" if ucoef is not None else "solver" if scoef is not None else \
                 "plms" if pcoef is not None else "ddim"
-            if sched == "plms" and noise_fn is not None:
+            if noise_fn is not None and randn_draws is not None:
+                raise ValueError("noise_fn and randn_draws are exclusive: pass one")
+            stochastic = noise_fn is not None or randn_draws is not None
+            if sched == "plms" and stochastic:
                 raise NotImplementedError("PNDM has no stochastic step: noise_fn is DDIM / solver-only")
-            if sched == "unipc" and (noise_fn is not None or blend is not None):
+            if sched == "unipc" and (stochastic or blend is not None):
                 raise NotImplementedError("eta / the 4-channel blend are DDIM-only on the fused path")
             if sched == "solver" and blend is not None:
                 raise NotImplementedError("the 4-channel blend is DDIM-only on the fused path")
             st = self._get(B, h, w, do_cfg, prompt_embeds.shape[1], noise_fn is not None, extra_per_copy, sched,
-                           blend is not None, bool(guess_mode) and K > 0)
+                           blend is not None, bool(guess_mode) and K > 0, randn_draws is not None)
+            if randn_draws is not None:
+                if any(not (0 <= d[4] and d[4] + d[5] <= B) for d in randn_draws):
+                    raise ValueError(f"randn_draws: rows outside the {B} latent rows")
+                st["draws"].copy_(ops.randn_draw_bytes(randn_draws, B).to(dev))
             if sched == "unipc":
                 if len(ucoef) != n_steps:
                     raise ValueError("ucoef needs one row per step")
@@ -364,19 +380,19 @@ def _upload(dst: torch.Tensor, src: torch.Tensor) -> None:
     """dst <- src without a host synchronisation: a host tensor is staged in pinned memory and copied asynchronously
     (the pinned block is not reused before the copy has run)"""
     if src.device.type == "cpu":
-        src = src.to(torch.float32).contiguous().pin_memory()
+        src = src.to(dst.dtype).contiguous().pin_memory()
         dst.copy_(src, non_blocking=True)
     else:
         dst.copy_(src)
 
 
 class SlottedPlan:
-    """One step program over S slots, each an independent request with its own step count, guidance scale, inputs and
-    side-net scale. Slot s owns the UNet rows 2s (unconditional) and 2s + 1 (conditional): the CFG pair of a slot is
+    """One step program over S slots, each an independent request with its own step count, guidance scale, inputs,
+    side-net scale and, for DDIM with eta > 0 and the stochastic solvers, its own device-drawn noise. Slot s owns the UNet rows 2s (unconditional) and 2s + 1 (conditional): the CFG pair of a slot is
     contiguous, so every step kernel runs unchanged on one slot (batch 1, two copies of the next input).
 
     Per slot the device holds a timestep table, an 8-float coefficient table (guidance in column 5), a side-net
-    scale x keep table, a step counter and the scheduler state. Each replay records, besides the shared nets, one time
+    scale x keep table, a step counter, the scheduler state and one pp_randn_draw entry (batch 1). Each replay records, besides the shared nets, one time
     embedding per slot, one step launch per slot (advancing that slot's counter) and, for a side net, one zero-conv
     launch per slot and residual. `admit` loads a request's loop inputs (what the pipeline hands `FusedDenoiser.run`)
     into a slot, `hold` parks a slot on rows that keep its latents fixed, `replay(k)` runs k steps of every slot."""
@@ -398,6 +414,9 @@ class SlottedPlan:
         self.coef = torch.zeros(S, MAX_STEPS, 8, **f32)
         self.side_scale = torch.zeros(S, MAX_STEPS, 1, **f32)
         self.latents = torch.zeros(S, hw, 4, **f32)
+        # the ddim / solver step launches always carry their slot's draw entry: a slot whose step has sigma / r[5]
+        # equal to 0 (deterministic requests, the hold rows) draws nothing, so one plan serves every request
+        self.draws = torch.zeros(S, ops.RANDN_DRAW_BYTES, dtype=torch.uint8, device=dev)
         self.pool = pool = Pool(dev)
         steps = [(self.timesteps[s], self.step_idx[s:s + 1]) for s in range(S)]
         common = dict(pool=pool, program=self.program, ctx_program=self.ctx_program, steps=steps)
@@ -437,11 +456,12 @@ class SlottedPlan:
                 self.program.add(ops.unipc_desc(**slot, last_sample=st["last_sample"], m1=st["m1"], m2=st["m2"],
                                                 ucoef=st["ucoef"]))
             elif sched == "solver":
-                self.program.add(ops.solver_desc(**slot, m1=st["m1"], scoef=st["scoef"]))
+                self.program.add(ops.solver_desc(**slot, m1=st["m1"], scoef=st["scoef"], draws=self.draws[s]))
             elif sched == "plms":
                 self.program.add(ops.plms_desc(**slot, cur_sample=st["cur_sample"], ets=st["ets"], pcoef=st["pcoef"]))
             else:
-                self.program.add(ops.cfg_ddim_desc(**slot, noise=None, guidance_scale=0.0, guidance_from_coef=True))
+                self.program.add(ops.cfg_ddim_desc(**slot, noise=None, draws=self.draws[s], guidance_scale=0.0,
+                                                   guidance_from_coef=True))
         self.bytes = pool.bytes
         self.graph = False
         # the hold rows of every table, on the device: parking a slot is a device-to-device copy
@@ -472,12 +492,15 @@ class SlottedPlan:
 
     def admit(self, s: int, *, latents, prompt_embeds, timesteps, coef, guidance_scale, extra=None,
               side_prompt_embeds=None, control_image=None, side_scale=1.0, side_keep=None, noise_fn=None, ucoef=None,
-              scoef=None, pcoef=None, blend=None, callback=None, guess_mode=False) -> int:
+              scoef=None, pcoef=None, blend=None, callback=None, guess_mode=False, randn_draws=None) -> int:
         """load one request's loop inputs (the keywords the pipelines pass `FusedDenoiser.run`, for one image under
         classifier-free guidance) into slot s and re-run the per-prompt programs; returns the request's step count"""
         h, w, dev = self.h, self.w, self.x_in.device
         if noise_fn is not None or blend is not None or callback is not None or guess_mode:
-            raise NotImplementedError("slots take no per-step noise, 4-channel blend, callback or guess mode")
+            raise NotImplementedError("slots take no host-drawn noise, 4-channel blend, callback or guess mode")
+        if randn_draws is not None and (self.sched not in ("ddim", "solver") or len(randn_draws) != 1
+                                        or tuple(randn_draws[0][4:]) != (0, 1)):
+            raise ValueError("a slot's device-drawn noise is one draw of its one latent row (DDIM / solver plans)")
         if tuple(latents.shape) != (1, 4, h, w) or prompt_embeds.shape[0] != 2:
             raise ValueError(f"a slot takes one {h}x{w} latent and its [negative; positive] prompt rows")
         given = {"ucoef": ucoef, "scoef": scoef, "pcoef": pcoef}
@@ -526,6 +549,7 @@ class SlottedPlan:
                 ci = self.side_plan.inputs["cond_in"]
                 ci[rows].copy_(ops.nchw_to_nhwc(img.to(dev).float().contiguous(), ci.shape[-1]).view_as(ci[rows]))
                 self.side_plan.cond_program.run()
+        _upload(self.draws[s], ops.randn_draw_bytes(randn_draws or [], 1))
         self.ctx_program.run()
         self.reset_counter(s)
         return n

@@ -251,10 +251,37 @@ def gn_desc(*, x0, x1, c0, c1, batch, hw, groups, gamma, beta, eps, silu, y, sta
     return Desc("gn", g, (x0, x1, gamma, beta, stats, y, part0, part1))
 
 
+RANDN_DRAW_BYTES = C.sizeof(N.RandnDraw)
+
+
+def randn_draw_bytes(draws, n: int) -> torch.Tensor:
+    """`n` pp_randn_draw entries as a uint8 host tensor: `draws` (tuples in the field order of `_native.RandnDraw`)
+    first, then entries that match no row"""
+    if len(draws) > n:
+        raise ValueError(f"{len(draws)} draws for a table of {n}")
+    arr = (N.RandnDraw * n)()
+    for k, d in enumerate(draws):
+        arr[k] = N.RandnDraw(*d)
+    return torch.frombuffer(bytearray(arr), dtype=torch.uint8)
+
+
+def _draws(table, noise):
+    """(pointer, count) of a draw table (uint8 tensor of whole pp_randn_draw entries)"""
+    if table is None:
+        return None, 0
+    if noise is not None:
+        raise ValueError("noise and draws are exclusive")
+    if table.dtype != torch.uint8 or table.numel() % RANDN_DRAW_BYTES or not table.is_contiguous():
+        raise ValueError("draws: a contiguous uint8 table of whole pp_randn_draw entries")
+    return N.ptr(table), table.numel() // RANDN_DRAW_BYTES
+
+
 def cfg_ddim_desc(*, eps, eps_fp32, eps_ld, latents, coef, step_idx, advance_step, noise,
                   guidance_scale, do_cfg, batch, hw, next_in=None, next_c=0, n_copies=0,
                   extra=None, extra_c=0, guidance_from_coef=False, extra_per_copy=False, blend_x0=None,
-                  blend_mask=None, blend_noise=None) -> Desc:
+                  blend_mask=None, blend_noise=None, draws=None) -> Desc:
+    """pp_cfg_ddim_step (include/powerpaint_b200.h); `draws`: a device uint8 table of pp_randn_draw entries
+    (`randn_draw_bytes`), the variance noise drawn in the kernel (exclusive with `noise`)"""
     d = N.CfgDdimDesc()
     d.eps, d.eps_fp32, d.eps_ld = N.ptr(eps), 1 if eps_fp32 else 0, eps_ld
     d.latents, d.coef, d.step_idx = N.ptr(latents), N.ptr(coef), N.ptr(step_idx)
@@ -267,7 +294,9 @@ def cfg_ddim_desc(*, eps, eps_fp32, eps_ld, latents, coef, step_idx, advance_ste
     d.guidance_from_coef = 1 if guidance_from_coef else 0
     d.extra_per_copy = 1 if extra_per_copy else 0
     d.blend_x0, d.blend_mask, d.blend_noise = N.ptr(blend_x0), N.ptr(blend_mask), N.ptr(blend_noise)
-    return Desc("cfg_ddim", d, (eps, latents, coef, step_idx, noise, next_in, extra, blend_x0, blend_mask, blend_noise))
+    d.draws, d.n_draws = _draws(draws, noise)
+    return Desc("cfg_ddim", d, (eps, latents, coef, step_idx, noise, next_in, extra, blend_x0, blend_mask, blend_noise,
+                                draws))
 
 
 def unipc_desc(*, eps, eps_fp32, eps_ld, latents, last_sample, m1, m2, coef, ucoef, step_idx, advance_step, do_cfg,
@@ -283,8 +312,9 @@ def unipc_desc(*, eps, eps_fp32, eps_ld, latents, last_sample, m1, m2, coef, uco
 
 
 def solver_desc(*, eps, eps_fp32, eps_ld, latents, m1, coef, scoef, step_idx, advance_step, do_cfg, batch, hw,
-                noise=None, next_in=None, next_c=0, n_copies=0) -> Desc:
-    """pp_solver_step (include/powerpaint_b200.h): CFG + one folded DPM-Solver++ / Euler / Euler-ancestral step"""
+                noise=None, next_in=None, next_c=0, n_copies=0, draws=None) -> Desc:
+    """pp_solver_step (include/powerpaint_b200.h): CFG + one folded DPM-Solver++ / Euler / Euler-ancestral step;
+    `draws` as in `cfg_ddim_desc`"""
     d = N.SolverDesc()
     d.eps, d.eps_fp32, d.eps_ld = N.ptr(eps), 1 if eps_fp32 else 0, eps_ld
     d.latents, d.m1, d.noise = N.ptr(latents), N.ptr(m1), N.ptr(noise)
@@ -292,7 +322,8 @@ def solver_desc(*, eps, eps_fp32, eps_ld, latents, m1, coef, scoef, step_idx, ad
     d.advance_step, d.do_cfg = 1 if advance_step else 0, 1 if do_cfg else 0
     d.batch, d.hw = batch, hw
     d.next_in, d.next_c, d.n_copies = N.ptr(next_in), next_c, n_copies
-    return Desc("solver", d, (eps, latents, m1, noise, coef, scoef, step_idx, next_in))
+    d.draws, d.n_draws = _draws(draws, noise)
+    return Desc("solver", d, (eps, latents, m1, noise, coef, scoef, step_idx, next_in, draws))
 
 
 def plms_desc(*, eps, eps_fp32, eps_ld, latents, cur_sample, ets, coef, pcoef, step_idx, advance_step, do_cfg,

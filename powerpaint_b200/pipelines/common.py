@@ -8,7 +8,7 @@ Restated from the reference: `prepare_mask_and_masked_image`
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Callable, List, Optional, Union
+from typing import Callable, List, Optional, Tuple, Union
 
 import numpy as np
 import PIL.Image
@@ -67,22 +67,96 @@ def randn_tensor(shape, generator=None, device=None, dtype=None):
     return torch.randn(shape, generator=generator, device=rand_device, dtype=dtype).to(device)
 
 
-def solver_loop_inputs(scheduler, timesteps, shape, generator, device):
-    """(scoef, noise_fn, finish) for a scheduler stepped by `pp_solver_step` (kind "solver") over `timesteps`, a
-    suffix of `scheduler.timesteps` (strength < 1). diffusers' `step` draws `randn_tensor(model_output.shape)` once
-    per call: the stochastic variants consume that noise through `noise_fn(i)` (in step order), while Euler's
-    discarded draws are made by `finish()` after the loop, so the generator ends where the reference leaves it."""
-    scoef = scheduler.solver_coefficients(first=len(scheduler.timesteps) - len(timesteps))
+RANDN_BLOCK = 256  # torch's block size for CUDA distribution kernels (`block_size_bound`)
 
-    def draw(i):
+
+def randn_policy(numel: int, sms: int, max_threads_per_sm: int) -> Tuple[int, int]:
+    """(threads, Philox offset increment) of torch's CUDA `randn` of `numel` fp32 elements on a device with `sms`
+    multiprocessors (`calc_execution_policy`, ATen/native/cuda/DistributionTemplates.h): blocks of 256, the grid
+    capped at sms * (max_threads_per_sm / 256), four elements per thread and pass (one curand_normal4), and four
+    counter values per pass"""
+    grid = min((numel + RANDN_BLOCK - 1) // RANDN_BLOCK, sms * (max_threads_per_sm // RANDN_BLOCK))
+    threads = RANDN_BLOCK * grid
+    return threads, ((numel - 1) // (threads * 4) + 1) * 4
+
+
+def _device_policy(index: int) -> Tuple[int, int]:
+    """(multiprocessors, max threads per multiprocessor) of CUDA device `index`: the numbers torch's policy reads"""
+    p = torch.cuda.get_device_properties(index)
+    return p.multi_processor_count, p.max_threads_per_multi_processor
+
+
+def _default_generator(index: int):
+    return torch.cuda.default_generators[index]
+
+
+def device_randn_draws(generator, shape, device, n_draws: int) -> Optional[List[tuple]]:
+    """The draw-table rows (`pp_randn_draw` field tuples: seed, offset0, offset_per_step, threads, first_row, rows)
+    that let the step kernels compute, at step i of a loop on `device`, exactly what the (i + 1)-th
+    `randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)` from here would draw; each
+    generator's stream is reserved past `n_draws` such draws, so afterwards it stands where those draws leave it.
+
+    The device path takes a CUDA generator on `device`, a list of them (one draw of shape (1, ...) per latent row,
+    as `randn_tensor` does), or None (the device's default CUDA generator). Everything else returns None and keeps
+    the host path: CPU generators (their mt19937 stream), a CPU device, a generator on another device, and a list
+    that holds one generator twice (its rows interleave their draws)."""
+    device = torch.device(device)
+    if device.type != "cuda" or len(shape) != 4 or shape[1] != 4:
+        return None
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    if isinstance(generator, list) and len(generator) == 1:
+        generator = generator[0]
+    gens = generator if isinstance(generator, list) else [generator if generator is not None
+                                                            else _default_generator(index)]
+    if isinstance(generator, list) and len(generator) != shape[0]:
+        return None
+    for g in gens:
+        dev = torch.device(g.device)
+        if dev.type != "cuda" or (dev.index if dev.index is not None else torch.cuda.current_device()) != index:
+            return None
+    if len({id(g) for g in gens}) != len(gens):
+        return None
+    rows = shape[0] // len(gens)
+    threads, per_step = randn_policy(rows * int(np.prod(shape[1:])), *_device_policy(index))
+    out = []
+    for k, g in enumerate(gens):
+        off = g.get_offset()
+        g.set_offset(off + n_draws * per_step)
+        out.append((g.initial_seed(), off, per_step, threads, k * rows, rows))
+    return out
+
+
+def step_noise(generator, shape, device, n_steps: int) -> dict:
+    """the `FusedDenoiser.run` keyword that gives each of `n_steps` stochastic steps the noise the reference draws
+    with `randn_tensor(shape, generator, device, float32)`: `randn_draws` when the kernels can draw it
+    (`device_randn_draws`, the stream then reserved), else `noise_fn(i)`, drawn on the host every step"""
+    draws = device_randn_draws(generator, shape, device, n_steps)
+    if draws is not None:
+        return {"randn_draws": draws}
+
+    def noise_fn(i):
         return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+    return {"noise_fn": noise_fn}
 
-    def finish():
-        if scheduler.draws_noise and not scheduler.stochastic:
-            for i in range(len(timesteps)):
-                draw(i)
 
-    return scoef, (draw if scheduler.stochastic else None), finish
+def solver_loop_inputs(scheduler, timesteps, shape, generator, device):
+    """(scoef, noise, finish) for a scheduler stepped by `pp_solver_step` (kind "solver") over `timesteps`, a
+    suffix of `scheduler.timesteps` (strength < 1). diffusers' `step` draws `randn_tensor(model_output.shape)` once
+    per call: the stochastic variants consume that noise through `noise` (the `step_noise` keyword, in step order),
+    while Euler's discarded draws are made by `finish()` after the loop, or reserved at once on the device path, so
+    the generator ends where the reference leaves it."""
+    scoef = scheduler.solver_coefficients(first=len(scheduler.timesteps) - len(timesteps))
+    if not scheduler.draws_noise:
+        return scoef, {}, None
+    if not scheduler.stochastic:
+        if device_randn_draws(generator, shape, device, len(timesteps)) is not None:
+            return scoef, {}, None
+
+        def finish():
+            for _ in range(len(timesteps)):
+                randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+        return scoef, {}, finish
+    return scoef, step_noise(generator, shape, device, len(timesteps)), None
 
 
 def callback_fires(i: int, n_timesteps: int, num_warmup_steps: int, order: int) -> bool:

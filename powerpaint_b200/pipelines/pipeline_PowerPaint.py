@@ -20,7 +20,7 @@ import torch
 from ..denoise import FusedDenoiser
 from ..models import AutoencoderKL, BrushNetModel, ControlNetModel, UNet2DConditionModel
 from .common import (LoopInputs, callback_fires, decode_latents, encode_text, prepare_mask_and_masked_image, run_loop,
-                     randn_tensor, solver_loop_inputs, uint8_device_inputs, vae_encode)
+                     randn_tensor, solver_loop_inputs, step_noise, uint8_device_inputs, vae_encode)
 
 # the components stored as diffusers model directories, by their name in model_index.json
 _MODEL_COMPONENTS = {"unet": UNet2DConditionModel, "brushnet": BrushNetModel, "controlnet": ControlNetModel,
@@ -452,14 +452,11 @@ class StableDiffusionInpaintPipeline:
             sqrt_alpha = [float(ac[int(timesteps[i + 1])]) ** 0.5 if i < len(timesteps) - 1 else 1.0
                           for i in range(len(timesteps))]
             blend = dict(x0=image_latents, mask=mask, noise=noise, sqrt_alpha=sqrt_alpha)
-        noise_fn = None
+        noise_kw = {}
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
-            shape = latents.shape
-
-            def noise_fn(i):
-                return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+            noise_kw = step_noise(generator, latents.shape, device, len(timesteps))
         if kind == "solver":
-            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
+            scoef, noise_kw, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
             n_ts = len(timesteps)
@@ -471,9 +468,10 @@ class StableDiffusionInpaintPipeline:
                 return None
         # `scoef` / `pcoef` are passed only when such a scheduler is set: a denoiser whose `run` predates those kinds
         # keeps serving DDIM and UniPC unchanged
-        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
+        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef), ("randn_draws", noise_kw.get("randn_draws")))
+               if v is not None}
         run = dict(latents=latents, prompt_embeds=prompt_embeds, timesteps=timesteps, coef=coef,
                    guidance_scale=guidance_scale,
                    extra=torch.cat([mask, masked_image_latents], dim=1) if num_channels_unet == 9 else None,
-                   noise_fn=noise_fn, ucoef=ucoef, blend=blend, callback=cb, **opt)
+                   noise_fn=noise_kw.get("noise_fn"), ucoef=ucoef, blend=blend, callback=cb, **opt)
         return LoopInputs(run, finish, output_type, return_dict)

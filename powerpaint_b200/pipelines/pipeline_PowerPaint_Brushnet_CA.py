@@ -21,7 +21,7 @@ import torch
 from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import BrushNetModel, UNet2DConditionModel
 from .common import (LoopInputs, callback_fires, check_control_guidance, check_image, check_prompt_arguments,
-                     encode_text, preprocess_image, randn_tensor,
+                     encode_text, preprocess_image, randn_tensor, step_noise,
                      solver_loop_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
@@ -292,12 +292,11 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
         ucoef = self.scheduler.unipc_coefficients() if kind == "unipc" else None
         pcoef = self.scheduler.plms_coefficients() if kind == "plms" else None
         scoef = finish = None
-        noise_fn = None
+        noise_kw = {}
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
-            def noise_fn(i):
-                return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+            noise_kw = step_noise(generator, shape, device, len(ts))
         if kind == "solver":
-            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, ts, shape, generator, device)
+            scoef, noise_kw, finish = solver_loop_inputs(self.scheduler, ts, shape, generator, device)
         cb = None
         if callback_on_step_end is not None or callback is not None:
             pipe = self
@@ -325,11 +324,12 @@ class StableDiffusionPowerPaintBrushNetPipeline(StableDiffusionInpaintPipeline):
                 return new
         # `scoef` / `guess_mode` are passed only when set: a denoiser whose `run` predates them keeps serving DDIM
         # and UniPC unchanged
-        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef)) if v is not None}
+        opt = {k: v for k, v in (("scoef", scoef), ("pcoef", pcoef), ("randn_draws", noise_kw.get("randn_draws")))
+               if v is not None}
         if guess_mode:
             opt["guess_mode"] = True
         run = dict(latents=latents, prompt_embeds=prompt_embedsU, side_prompt_embeds=prompt_embeds, timesteps=ts,
                    coef=coef, guidance_scale=guidance_scale, extra=conditioning_latents,
-                   side_scale=float(brushnet_conditioning_scale), side_keep=keep, ucoef=ucoef, noise_fn=noise_fn,
+                   side_scale=float(brushnet_conditioning_scale), side_keep=keep, ucoef=ucoef, noise_fn=noise_kw.get("noise_fn"),
                    callback=cb, **opt)
         return LoopInputs(run, finish, output_type, return_dict)

@@ -21,7 +21,7 @@ from ..denoise import FusedDenoiser
 from ..models.unet_2d_condition import ControlNetModel, MultiControlNetModel, UNet2DConditionModel
 from .common import (LoopInputs, callback_fires, check_control_guidance, check_image, check_prompt_arguments,
                      prepare_mask_and_masked_image, preprocess_image,
-                     randn_tensor, solver_loop_inputs, uint8_device_inputs)
+                     randn_tensor, solver_loop_inputs, step_noise, uint8_device_inputs)
 from .pipeline_PowerPaint import StableDiffusionInpaintPipeline
 
 logger = logging.getLogger(__name__)
@@ -206,14 +206,11 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             ucoef = self.scheduler.unipc_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
         if kind == "plms":
             pcoef = self.scheduler.plms_coefficients(first=len(self.scheduler.timesteps) - len(timesteps))
-        noise_fn = None
+        noise_kw = {}
         if eta > 0 and "eta" in extra_step_kwargs:  # schedulers without `eta` ignore it (signature sniffing, :536-551)
-            shape = latents.shape
-
-            def noise_fn(i):
-                return randn_tensor(shape, generator=generator, device=device, dtype=torch.float32)
+            noise_kw = step_noise(generator, latents.shape, device, len(timesteps))
         if kind == "solver":
-            scoef, noise_fn, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
+            scoef, noise_kw, finish = solver_loop_inputs(self.scheduler, timesteps, latents.shape, generator, device)
         cb = None
         if callback is not None:
             n_ts = len(timesteps)
@@ -239,7 +236,9 @@ class StableDiffusionControlNetInpaintPipeline(StableDiffusionInpaintPipeline):
             side["scoef"] = scoef
         if pcoef is not None:
             side["pcoef"] = pcoef
+        if "randn_draws" in noise_kw:
+            side["randn_draws"] = noise_kw["randn_draws"]
         run = dict(latents=latents, prompt_embeds=prompt_embeds, side_prompt_embeds=prompt_embeds, timesteps=timesteps,
                    coef=coef, guidance_scale=guidance_scale, extra=torch.cat([mask, masked_image_latents], dim=1),
-                   noise_fn=noise_fn, ucoef=ucoef, callback=cb, **side)
+                   noise_fn=noise_kw.get("noise_fn"), ucoef=ucoef, callback=cb, **side)
         return LoopInputs(run, finish, output_type, return_dict)

@@ -11,8 +11,9 @@ replays the host swaps requests in and out:
   3. retire the slots that finished: decode their latents and complete their requests.
 
 Idle slots sit on hold rows (their latents do not move) and their counters are reset at every boundary, so no slot
-ever reads past its tables. Options that need the host inside the loop, or rows the slots do not have, are refused
-when the request is submitted.
+ever reads past its tables. DDIM with eta > 0 and the stochastic schedulers draw each slot's noise inside the step
+kernels from the request's CUDA generator. Options that need the host inside the loop, or rows the slots do not have,
+are refused when the request is submitted.
 """
 from __future__ import annotations
 
@@ -237,15 +238,30 @@ class RequestBatcher:
             return []
         return list(side.nets) if hasattr(side, "nets") else list(side) if isinstance(side, (list, tuple)) else [side]
 
+    def _cuda_generator(self, g) -> bool:
+        """`g` is one torch.Generator on the pipeline's CUDA device"""
+        if not isinstance(g, torch.Generator) or g.device.type != "cuda":
+            return False
+        dev = getattr(self.pipe.unet, "device", None)
+        if dev is None:
+            return True
+        dev = torch.device(dev)
+        cur = torch.cuda.current_device
+        return dev.type == "cuda" and (g.device.index if g.device.index is not None else cur()) == \
+            (dev.index if dev.index is not None else cur())
+
     def check(self, kwargs: dict) -> None:
         """raise for a request the slots cannot serve"""
         def refuse(msg):
             raise NotImplementedError(f"RequestBatcher: {msg}")
-        if float(kwargs.get("eta", 0.0) or 0.0) > 0:
-            refuse("`eta` > 0 draws noise on the host every step")
+        # the step kernels draw a slot's noise from its generator's Philox stream: that takes one CUDA generator on
+        # the pipeline's device; any other generator's noise would be drawn on the host every step
+        eta = float(kwargs.get("eta", 0.0) or 0.0) > 0
         sch = self.pipe.scheduler
-        if getattr(sch, "stochastic", False):
-            refuse(f"the stochastic scheduler {type(sch).__name__} draws noise on the host every step")
+        if (eta or getattr(sch, "stochastic", False)) and not self._cuda_generator(kwargs.get("generator")):
+            what = "`eta` > 0" if eta else f"the stochastic scheduler {type(sch).__name__}"
+            refuse(f"{what} draws noise on the host every step and needs a CUDA generator: pass one `torch.Generator` "
+                   "on the pipeline's CUDA device")
         for k in ("callback", "callback_on_step_end"):
             if kwargs.get(k) is not None:
                 refuse(f"`{k}` runs on the host inside the loop")
