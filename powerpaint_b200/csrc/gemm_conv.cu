@@ -20,8 +20,8 @@
 //  * Pipeline: persistent kernel, one 288-thread CTA per SM. Warp 8 = TMA producer; warps 0..7 = two consumer
 //    warpgroups, each issuing the wgmma.mma_async of 64 rows of the 128 x BLOCK_N tile and then running the epilogue
 //    of those rows. STAGES-deep smem ring with full/empty mbarriers that keeps running across tile boundaries, so the
-//    producer streams the next tile's operands while the consumers run this tile's epilogue. The accumulators go
-//    through a shared-memory fp32 tile (row per epilogue thread) that shares its space with the output staging tile.
+//    producer streams the next tile's operands while the consumers run this tile's epilogue. Each thread finishes its
+//    own accumulators in the wgmma fragment layout and writes the results to the output staging tile with stmatrix.
 //  * Split-K x2 (few tiles, long K): two CTAs per tile each stream half of K; the second hands its fp32 partial tile
 //    to the first through a global workspace (see the comment at the kernel).
 //  * Epilogue (fused): + bias[n] + time-embedding row vector + residual (skip / shortcut)
@@ -152,116 +152,52 @@ struct TileWalk {
     }
 };
 
-// Epilogue for 8 consecutive output columns of one row. v[] holds the accumulators; `sbias` points
-// at this tile's bias staged in shared memory (column n0 - n_base), r1/r2 hold the 8 bf16 residual
-// values that were loaded ahead of time (vector path only).
-template <bool kVec>
-__device__ __forceinline__ void epilogue_store8(const GemmKParams& p, float alpha, float (&v)[8], int64_t row, int grp,
-                                                int n0, const float* sbias, uint4 r1, uint4 r2) {
-    if (p.bias) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] += sbias[j];
-    }
-    if (p.rowvec) {
-        const float* rv = p.rowvec + (int64_t)grp * p.rowvec_ld + n0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-            if (kVec || n0 + j < p.N) v[j] += __ldg(rv + j);
-    }
-    if (p.res1) {
-        if (kVec) {
-            v[0] += bf16_lo(r1.x); v[1] += bf16_hi(r1.x); v[2] += bf16_lo(r1.y); v[3] += bf16_hi(r1.y);
-            v[4] += bf16_lo(r1.z); v[5] += bf16_hi(r1.z); v[6] += bf16_lo(r1.w); v[7] += bf16_hi(r1.w);
-        } else {
-            const __nv_bfloat16* r = p.res1 + row * p.ldr1 + n0;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (n0 + j < p.N) v[j] += __bfloat162float(r[j]);
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] *= alpha;
-    if (p.res2) {
-        if (kVec) {
-            v[0] += bf16_lo(r2.x); v[1] += bf16_hi(r2.x); v[2] += bf16_lo(r2.y); v[3] += bf16_hi(r2.y);
-            v[4] += bf16_lo(r2.z); v[5] += bf16_hi(r2.z); v[6] += bf16_lo(r2.w); v[7] += bf16_hi(r2.w);
-        } else {
-            const __nv_bfloat16* r = p.res2 + row * p.ldr2 + n0;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (n0 + j < p.N) v[j] += __bfloat162float(r[j]);
-        }
-    }
-    if (p.act != PP_ACT_NONE) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = apply_act(v[j], p.act);
-    }
+// Generic epilogue of one output element (mode 1: fp32 / transposed / ragged N; the caller checks the row and n < N).
+// `bias` is the staged bias of column n.
+__device__ __forceinline__ void epilogue_store1(const GemmKParams& p, float alpha, float v, int64_t row, int grp, int n,
+                                                float bias) {
+    if (p.bias) v += bias;
+    if (p.rowvec) v += __ldg(p.rowvec + (int64_t)grp * p.rowvec_ld + n);
+    if (p.res1) v += __bfloat162float(p.res1[row * p.ldr1 + n]);
+    v *= alpha;
+    if (p.res2) v += __bfloat162float(p.res2[row * p.ldr2 + n]);
+    if (p.act != PP_ACT_NONE) v = apply_act(v, p.act);
     if (p.epilogue == PP_EPI_TRANSPOSED) {
-        // out[(row / t_rows) * N + n][row % t_rows]; lanes of a warp hold consecutive rows,
-        // so each per-column store is a 64-byte contiguous run across the warp.
+        // out[(row / t_rows) * N + n][row % t_rows]
         const int64_t b = (int)row / p.t_rows;  // 32-bit: a 64-bit division is a subroutine call, which would serialise the wgmma pipeline
         const int64_t t = row - b * p.t_rows;
-        if (p.t_fp16) {
-            __half* o = reinterpret_cast<__half*>(p.out) + (b * p.N + n0) * p.t_ld + t;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (kVec || n0 + j < p.N) o[(int64_t)j * p.t_ld] = __float2half_rn(v[j]);
-            return;
-        }
-        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + (b * p.N + n0) * p.t_ld + t;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-            if (kVec || n0 + j < p.N) o[(int64_t)j * p.t_ld] = __float2bfloat16_rn(v[j]);
-        return;
-    }
-    if (p.out_fp32) {
-        float* o = reinterpret_cast<float*>(p.out) + row * p.ldc + n0;
-        if (kVec) {
-            *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-            *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (n0 + j < p.N) o[j] = v[j];
-        }
+        if (p.t_fp16) reinterpret_cast<__half*>(p.out)[(b * p.N + n) * p.t_ld + t] = __float2half_rn(v);
+        else reinterpret_cast<__nv_bfloat16*>(p.out)[(b * p.N + n) * p.t_ld + t] = __float2bfloat16_rn(v);
+    } else if (p.out_fp32) {
+        reinterpret_cast<float*>(p.out)[row * p.ldc + n] = v;
     } else {
-        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + row * p.ldc + n0;
-        if (kVec) {
-            uint4 q;
-            q.x = pack_bf16x2(v[0], v[1]);
-            q.y = pack_bf16x2(v[2], v[3]);
-            q.z = pack_bf16x2(v[4], v[5]);
-            q.w = pack_bf16x2(v[6], v[7]);
-            *reinterpret_cast<uint4*>(o) = q;
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                if (n0 + j < p.N) o[j] = __float2bfloat16_rn(v[j]);
-        }
+        reinterpret_cast<__nv_bfloat16*>(p.out)[row * p.ldc + n] = __float2bfloat16_rn(v);
     }
 }
 
-// Accumulator tile in shared memory: fp32 rows of BLOCK_N + 4 floats (the pad spreads the row-per-thread reads over
-// the banks). Up to 160 columns it holds all 128 rows; the 256-wide tile holds the 64 rows of one warpgroup at a
-// time (the two warpgroups take turns), which leaves room for three ring stages.
-__host__ __device__ constexpr int acc_rows_for(int block_n) { return block_n == 256 ? 64 : 128; }
-__host__ __device__ constexpr int acc_ld_for(int block_n) { return block_n + 4; }
-// Output staging tile: the epilogue writes its accumulator rows (bf16) into shared memory laid out as the boxes
-// of a TMA store — 64-column sub-tiles [128 rows][128 B] with the 128-byte swizzle (the 160-wide tile ends in a
+// Four 8x8 16-bit matrices from the accumulator fragment into shared memory; lane l gives the address of row l % 8 of
+// matrix l / 8. With .trans each matrix is stored transposed (a fragment column becomes a row).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
+                 "r"(d)
+                 : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b),
+                 "r"(c), "r"(d)
+                 : "memory");
+}
+
+// Output staging tile: the epilogue writes its results (bf16) straight from the accumulator fragments (stmatrix) into
+// shared memory laid out as the boxes of a TMA store — 64-column sub-tiles [128 rows][128 B] with the 128-byte swizzle (the 160-wide tile ends in a
 // 32-column sub-tile [128][64 B] with the 64-byte swizzle) — and one thread per sub-tile hands them to the TMA unit,
 // which writes whole rows and clips whatever lies outside the tensor (ragged conv tiles, rows >= M, columns >= N).
 __host__ __device__ constexpr int out_stage_bytes_for(int block_n) {
     return (block_n / 64) * 16384 + (block_n % 64) * 256;
 }
-// the staging tile and the accumulator tile share one 1024-byte aligned region
-__host__ __device__ constexpr int acc_region_bytes_for(int block_n) {
-    return ((acc_rows_for(block_n) * acc_ld_for(block_n) * 4 > out_stage_bytes_for(block_n)
-                 ? acc_rows_for(block_n) * acc_ld_for(block_n) * 4
-                 : out_stage_bytes_for(block_n)) + 1023) / 1024 * 1024;
-}
 // fixed part: 1 KB alignment slack, barriers, bias + LayerNorm-sum staging [4][BLOCK_N] floats, row table
 __host__ __device__ constexpr int fixed_smem_for(int block_n) {
-    return 1024 + 256 + 4 * block_n * 4 + 128 * 8 + 1024 + acc_region_bytes_for(block_n);
+    return 1024 + 256 + 4 * block_n * 4 + 128 * 8 + 1024 + out_stage_bytes_for(block_n);
 }
 // as many ring stages as the per-block shared memory takes (at most 8)
 __host__ __device__ constexpr int stages_for(int block_n) {
@@ -273,15 +209,16 @@ __host__ __device__ constexpr int smem_bytes_for(int block_n) {
     return stages_for(block_n) * (A_STAGE_BYTES + block_n * BLOCK_K * 2) + fixed_smem_for(block_n);
 }
 static_assert(stages_for(256) >= 2 && smem_bytes_for(256) <= GEMM_SMEM_LIMIT, "256-wide tile does not fit");
-static_assert(stages_for(160) >= 3 && stages_for(128) >= 3 && stages_for(64) >= 3, "ring too shallow");
+static_assert(stages_for(160) == 5 && stages_for(128) == 5 && stages_for(256) == 3 && stages_for(64) == 8,
+              "ring stages per tile width");
 
 // Persistent, warp-specialised kernel: grid = min(#tiles, #SMs); each CTA walks tiles
 // blockIdx.x, blockIdx.x + gridDim.x, ... (n fastest, so CTAs running concurrently share A tiles
 // through L2 and the weights stay L2-resident).
 //   warp 8      TMA producer  (smem ring continues across tile boundaries)
 //   warps 0..7  two consumer warpgroups: warpgroup g issues the wgmma of tile rows [64 g, 64 g + 64) and then runs
-//               the epilogue of the same rows — each of its four warps takes 32 rows and one half of the columns
-//               (alternating 32-column chunks), reading its row of the accumulator tile in shared memory
+//               the epilogue of the same rows straight from the accumulator registers (a thread holds two rows, 8 apart,
+//               and two columns of every 8-column group)
 // MODE selects the epilogue flavour at compile time (keeps the hot epilogue short and the
 // instruction footprint small): 0 = bf16 row-major output, N % 8 == 0 (bias, rowvec, two residuals,
 // alpha, SiLU), 1 = generic (fp32 / transposed / ragged N), 2 = GEGLU, 3 = mode 0 emitting the per-row records of the
@@ -297,8 +234,6 @@ template <int BLOCK_N, int MODE, bool kSplitK = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid_constant__ GemmKParams p) {
     constexpr int STAGES = stages_for(BLOCK_N);
     constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
-    constexpr int ACC_ROWS = acc_rows_for(BLOCK_N), ACC_LD = acc_ld_for(BLOCK_N);
-    constexpr bool kAccShared = ACC_ROWS < BLOCK_M;  // the two warpgroups take turns in the accumulator tile
 
     extern __shared__ uint8_t smem_raw[];
     // mode 3 (LayerNorm-statistics producer): mailbox between the epilogue and the ticket-server lane, and the verdict
@@ -308,11 +243,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sA = smem_base;
     const uint32_t sB = sA + STAGES * A_STAGE_BYTES;
-    // accumulator tile / output staging tile (aliased), 1024-byte aligned
+    // output staging tile, 1024-byte aligned
     const uint32_t s_out_addr = sB + STAGES * B_STAGE_BYTES;
     uint8_t* s_out = smem_raw + (s_out_addr - smem_u32(smem_raw));
-    float* sacc = reinterpret_cast<float*>(s_out);
-    const uint32_t bar_base = s_out_addr + acc_region_bytes_for(BLOCK_N);
+    const uint32_t bar_base = s_out_addr + out_stage_bytes_for(BLOCK_N);
     // barriers: full[STAGES], empty[STAGES]
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
@@ -322,12 +256,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
     float* su_all = sbias_all + 2 * BLOCK_N;
     // validity of each tile row (statistics pass)
     long long* s_row = reinterpret_cast<long long*>(reinterpret_cast<uint8_t*>(sbias_all) + 4 * BLOCK_N * 4);
-    // 16-byte piece of row r holding columns [col, col + 8) of the staged tile
-    auto stage_ptr = [&](int r, int col) -> uint8_t* {
+    // offset in the staging tile of the 16-byte piece of row r holding columns [col, col + 8)
+    auto stage_off = [&](int r, int col) -> uint32_t {
         const int sub = col >> 6, c = (col & 63) >> 3;
         if ((BLOCK_N % 64) != 0 && sub == BLOCK_N / 64)  // 32-column remainder sub-tile, 64-byte swizzle
-            return s_out + sub * 16384 + r * 64 + ((c ^ ((r >> 1) & 3)) << 4);
-        return s_out + sub * 16384 + r * 128 + ((c ^ (r & 7)) << 4);
+            return sub * 16384 + r * 64 + ((c ^ ((r >> 1) & 3)) << 4);
+        return sub * 16384 + r * 128 + ((c ^ (r & 7)) << 4);
     };
 
     const int warp = threadIdx.x >> 5;
@@ -468,30 +402,23 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
         }
     } else {
         // ===================== consumer warpgroups: MMA + epilogue =====================
-        const int wg = warp >> 2;                         // warpgroup: tile rows [64 wg, 64 wg + 64)
-        const int quarter = (warp & 1) + 2 * wg;          // rows of this warp: [32*quarter, +32)
-        const int half = (warp >> 1) & 1;                 // which of the two warps sharing those rows
-        const int etid = threadIdx.x;        // 0..255 among the epilogue threads
-        const int r = quarter * 32 + (int)lane_id();
-        // this thread's row of the accumulator tile
-        const float* arow = sacc + (r - (kAccShared ? 64 * wg : 0)) * ACC_LD;
-        auto acc_ld = [](const float* src, auto& dst) {
-            constexpr int NV = sizeof(dst) / sizeof(dst[0]);
-#pragma unroll
-            for (int i = 0; i < NV; i += 4) {
-                const float4 v = *reinterpret_cast<const float4*>(src + i);
-                dst[i] = __float_as_uint(v.x); dst[i + 1] = __float_as_uint(v.y);
-                dst[i + 2] = __float_as_uint(v.z); dst[i + 3] = __float_as_uint(v.w);
-            }
-        };
-        const bool vec_ok = (p.N % 8 == 0);
+        const int wg = warp >> 2;  // warpgroup: tile rows [64 wg, 64 wg + 64)
+        const int etid = threadIdx.x;  // 0..255 among the epilogue threads
+        const int lane = (int)lane_id(), quad = lane & 3;
+        // this thread's accumulators (wgmma fragment): tile rows r0 (h = 0) and r0 + 8 (h = 1), and per 8-column group i
+        // the columns 8 i + 2 quad + {0, 1}: facc[4 i + 2 h + {0, 1}]
+        const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        // stmatrix.x4 of the 8-column groups (i, i + 1): matrix lane / 8 is (rows + 8 ((lane / 8) & 1), group i + lane / 16);
+        // this lane addresses its row lane % 8 (transposed: its column)
+        const int st_row = 64 * wg + 16 * (warp & 3) + 8 * ((lane >> 3) & 1);
+        const int st_grp = lane >> 4, st_j = lane & 7;
         auto epi_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(GEMM_EPI_WARPS * 32) : "memory"); };
-        // ---- main loop of one tile: this warpgroup's 64 x BLOCK_N accumulators, then into the accumulator tile
+        // ---- main loop of one tile: this warpgroup's 64 x BLOCK_N accumulators. `before_drain` runs ahead of the last
+        // wait, so global loads it issues overlap the final MMAs.
         int ks = 0;  // ring slot and its phase, carried across tiles (the producer's sequence)
         uint32_t kph = 0;
-        auto mainloop = [&](int m_tile, int n_tile) {
+        auto mainloop = [&](float (&facc)[BLOCK_N / 2], int m_tile, int n_tile, auto&& before_drain) {
             // zeroed here (not by the first MMA's scale-d): the registers are then dead between tiles
-            float facc[BLOCK_N / 2];
 #pragma unroll
             for (int i = 0; i < BLOCK_N / 2; ++i) facc[i] = 0.f;
             int prev = 0;
@@ -510,6 +437,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 prev = ks;
                 if (++ks == STAGES) { ks = 0; kph ^= 1u; }
             }
+            before_drain();
             wgmma_wait<0>();
             wgmma_fence_regs(facc);
             if (lane_id() == 0) mbar_arrive(empty_bar(prev));
@@ -525,27 +453,32 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                     *fl = 0;  // ready for the next launch
                 }
             }
-            // the accumulator tile shares its space with the staging tile: the TMA unit has read the previous tile out
-            // of it, and every epilogue thread is past its reads of it (statistics pass included)
+            // the epilogue writes the staging tile next: the TMA unit has read the previous tile out of it, and every
+            // epilogue thread is past its reads of it (statistics pass included)
             if constexpr (MODE != 1) {
                 if ((etid & 31) == 0) bulk_wait_read_all();
             }
             epi_sync();
-            if constexpr (kAccShared) {  // warpgroup 1 waits until warpgroup 0 has read its rows out
-                if (wg == 1) asm volatile("bar.sync 2, %0;" ::"n"(GEMM_EPI_WARPS * 32) : "memory");
-            }
-            {
-                const int w4 = warp & 3, l = (int)lane_id();
-                float* dst = sacc + ((kAccShared ? 0 : 64 * wg) + 16 * w4 + (l >> 2)) * ACC_LD + 2 * (l & 3);
+            if constexpr (kSplitK) {
+                // split-K: the donor's raw fp32 accumulators go to the workspace in fragment order ([tile][group][thread]
+                // float4, coalesced); the owner adds the donor's to its own (owner + donor, always in this order)
+                float4* ws = reinterpret_cast<float4*>(p.splitk_ws) +
+                             ((int64_t)m_tile * n_tiles + n_tile) * (BLOCK_M * BLOCK_N / 4) + etid;
+                if (khalf) {
 #pragma unroll
-                for (int i = 0; i < BLOCK_N / 8; ++i) {
-                    *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(facc[4 * i], facc[4 * i + 1]);
-                    *reinterpret_cast<float2*>(dst + 8 * ACC_LD + 8 * i) = make_float2(facc[4 * i + 2], facc[4 * i + 3]);
+                    for (int i = 0; i < BLOCK_N / 8; ++i)
+                        ws[i * (GEMM_EPI_WARPS * 32)] = make_float4(facc[4 * i], facc[4 * i + 1], facc[4 * i + 2], facc[4 * i + 3]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < BLOCK_N / 8; ++i) {
+                        const float4 pp = __ldcg(ws + i * (GEMM_EPI_WARPS * 32));
+                        facc[4 * i] = facc[4 * i] + pp.x;
+                        facc[4 * i + 1] = facc[4 * i + 1] + pp.y;
+                        facc[4 * i + 2] = facc[4 * i + 2] + pp.z;
+                        facc[4 * i + 3] = facc[4 * i + 3] + pp.w;
+                    }
                 }
             }
-            // the warpgroup's rows are complete (each warpgroup reads only the rows it wrote)
-            if (wg == 0) asm volatile("bar.sync 3, 128;" ::: "memory");
-            else asm volatile("bar.sync 4, 128;" ::: "memory");
         };
         auto load_bias = [&](int n_tile_of) -> float {
             const int n = n_tile_of * BLOCK_N + etid;
@@ -578,12 +511,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             }
         }
         epi_sync();
-        float2 ln_cur = make_float2(1.f, 0.f);  // {rstd, -rstd * mean} of this thread's row in the current tile
+        // {rstd, -rstd * mean} of this thread's two rows in the current tile
+        float2 ln_cur[2] = {make_float2(1.f, 0.f), make_float2(1.f, 0.f)};
         if (ln && walk_first < num_tiles) {
-            const int64_t row0 = (int64_t)tw.m * BLOCK_M + r;
-            if (row0 < p.M) ln_cur = __ldg(p.ln_stats + row0);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t row0 = (int64_t)tw.m * BLOCK_M + r0 + 8 * h;
+                if (row0 < p.M) ln_cur[h] = __ldg(p.ln_stats + row0);
+            }
         }
         // ---- mode 3: verdict of the ticket server for request number `seq`, and the fold of a row's records
+        // (one thread per row: quad lanes 0 / 1 fold rows r0 / r0 + 8)
         int64_t prev_row = 0;
         bool prev_valid = false;
         auto ticket_verdict = [&](int seq) -> int {
@@ -650,366 +588,293 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 else *du = 0.f;
             }
             if (etid == 0) GT(lt, 16);
-            // output row of this thread
-            bool valid;
-            int64_t row;
-            int grp;
+            // output rows of this thread (tile rows r0 and r0 + 8)
+            bool valid[2];
+            int64_t row[2];
+            int grp[2];
             if (p.a_mode == PP_A_MATRIX) {
-                row = (int64_t)m_tile * BLOCK_M + r;
-                valid = row < p.M;
-                grp = p.rowvec ? (int)row / p.rows_per_group : 0;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    row[h] = (int64_t)m_tile * BLOCK_M + r0 + 8 * h;
+                    valid[h] = row[h] < p.M;
+                    grp[h] = p.rowvec ? (int)row[h] / p.rows_per_group : 0;
+                }
             } else {
                 int x0, y0, nb0;
                 tile_origin(m_tile, x0, y0, nb0);
-                // bw, bh, bn are powers of two
-                const int ix = r & (p.bw - 1);
-                const int iy = (r >> p.bw_log2) & (p.bh - 1);
-                const int in = r >> (p.bw_log2 + p.bh_log2);
-                const int ox = x0 + ix, oy = y0 + iy, on = nb0 + in;
-                valid = in < p.bn && ox < p.wo && oy < p.ho && on < p.nb;
-                row = ((int64_t)on * p.ho + oy) * p.wo + ox;
-                grp = on;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    // bw, bh, bn are powers of two
+                    const int r = r0 + 8 * h;
+                    const int ix = r & (p.bw - 1);
+                    const int iy = (r >> p.bw_log2) & (p.bh - 1);
+                    const int in = r >> (p.bw_log2 + p.bh_log2);
+                    const int ox = x0 + ix, oy = y0 + iy, on = nb0 + in;
+                    valid[h] = in < p.bn && ox < p.wo && oy < p.ho && on < p.nb;
+                    row[h] = ((int64_t)on * p.ho + oy) * p.wo + ox;
+                    grp[h] = on;
+                }
             }
             if (etid == 0) GT(lt, 17);
             const int n_base = n_tile * BLOCK_N;
             // mode 5: this tile's columns are stored transposed ([channel][token], V^T for the attention kernel)
             const bool ttile = MODE == 5 && n_tile >= p.trans_first_tile;
-            // LayerNorm fold: acc' = ln_rs * acc + ln_nm * u[n] with {ln_rs, ln_nm} = {rstd, -rstd * mean} of this row, as
-            // left by the producer (row_final). The pair of the NEXT tile's row is fetched now, so that its global-memory
-            // latency is off the epilogue's serial path (a per-tile fold of the raw records cost ~2500 cycles a tile).
-            const float ln_rs = ln_cur.x, ln_nm = ln_cur.y;
+            // LayerNorm fold: acc' = ln_rs * acc + ln_nm * u[n] with {ln_rs, ln_nm} = {rstd, -rstd * mean} of the row, as
+            // left by the producer (row_final). The pairs of the NEXT tile's rows are fetched now, so that their
+            // global-memory latency is off the epilogue's serial path (a per-tile fold of the raw records cost ~2500
+            // cycles a tile).
+            const float ln_rs[2] = {ln_cur[0].x, ln_cur[1].x}, ln_nm[2] = {ln_cur[0].y, ln_cur[1].y};
             if (ln) {
-                const int64_t nrow = (int64_t)tw.m * BLOCK_M + r;  // tw is already at the next tile
-                ln_cur = (next_tile < num_tiles && nrow < p.M) ? __ldg(p.ln_stats + nrow) : make_float2(1.f, 0.f);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t nrow = (int64_t)tw.m * BLOCK_M + r0 + 8 * h;  // tw is already at the next tile
+                    ln_cur[h] = (next_tile < num_tiles && nrow < p.M) ? __ldg(p.ln_stats + nrow) : make_float2(1.f, 0.f);
+                }
             }
-            // The tile's results stay in registers (packed bf16, 8 columns per uint4) until every thread has read its
-            // row of the accumulator tile, whose space the staging tile reuses.
-            constexpr int PK_N = MODE == 2 ? BLOCK_N / 32 : MODE == 1 ? 1 : BLOCK_N / 16;
-            uint4 pk[PK_N];
+            float facc[BLOCK_N / 2];
             if constexpr (MODE == 2) {
+                // GEGLU: value column c and gate column c + BLOCK_N / 2 sit in the same thread (BLOCK_N / 2 is a multiple
+                // of 8); the HALF output columns are staged like a HALF-wide tile
                 constexpr int HALF = BLOCK_N / 2;
                 const int o_base = n_tile * HALF;  // output column of this tile
                 const int n_out = p.N / 2;
-                mainloop(m_tile, n_tile);
+                mainloop(facc, m_tile, n_tile, [] {});
+                if (etid == 0) GT(lt, 5);
 #pragma unroll
-                for (int k = 0; k < BLOCK_N / 64; ++k) {
-                    const int c0 = half * 16 + 32 * k;
-                    uint32_t ra[16], rg[16];
-                    acc_ld(arow + c0, ra);
-                    acc_ld(arow + HALF + c0, rg);
-                    pk[2 * k] = pk[2 * k + 1] = make_uint4(0u, 0u, 0u, 0u);
-                    if (valid && o_base + c0 < n_out) {
+                for (int k = 0; k < HALF / 16; ++k) {
+                    uint32_t q[4];  // stmatrix operands: (group 2k, row h = 0 / 1), (group 2k + 1, row h = 0 / 1)
 #pragma unroll
-                        for (int h8 = 0; h8 < 16; h8 += 8) {
-                            // bias (and, with the LayerNorm fold, the weight row sums) of the 8 value / 8 gate columns
-                            // as 16-byte shared-memory loads: scalar loads made this epilogue LSU-bound
-                            float ba[8], bg[8], ua[8], ug[8];
-                            *reinterpret_cast<float4*>(&ba[0]) = *reinterpret_cast<const float4*>(sbias + c0 + h8);
-                            *reinterpret_cast<float4*>(&ba[4]) = *reinterpret_cast<const float4*>(sbias + c0 + h8 + 4);
-                            *reinterpret_cast<float4*>(&bg[0]) = *reinterpret_cast<const float4*>(sbias + HALF + c0 + h8);
-                            *reinterpret_cast<float4*>(&bg[4]) = *reinterpret_cast<const float4*>(sbias + HALF + c0 + h8 + 4);
-                            if (ln) {
-                                *reinterpret_cast<float4*>(&ua[0]) = *reinterpret_cast<const float4*>(su + c0 + h8);
-                                *reinterpret_cast<float4*>(&ua[4]) = *reinterpret_cast<const float4*>(su + c0 + h8 + 4);
-                                *reinterpret_cast<float4*>(&ug[0]) = *reinterpret_cast<const float4*>(su + HALF + c0 + h8);
-                                *reinterpret_cast<float4*>(&ug[4]) = *reinterpret_cast<const float4*>(su + HALF + c0 + h8 + 4);
-                            }
-                            float v[8];
+                    for (int g = 0; g < 2; ++g) {
+                        const int i = 2 * k + g, c = 8 * i + 2 * quad;
+                        const float2 ba = *reinterpret_cast<const float2*>(sbias + c);
+                        const float2 bg = *reinterpret_cast<const float2*>(sbias + HALF + c);
+                        float2 ua = make_float2(0.f, 0.f), ug = make_float2(0.f, 0.f);
+                        if (ln) {
+                            ua = *reinterpret_cast<const float2*>(su + c);
+                            ug = *reinterpret_cast<const float2*>(su + HALF + c);
+                        }
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float a = __uint_as_float(ra[h8 + j]), g = __uint_as_float(rg[h8 + j]);
+                        for (int h = 0; h < 2; ++h) {
+                            float v[2];
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                float a = facc[4 * i + 2 * h + e], gt = facc[4 * (i + HALF / 8) + 2 * h + e];
+                                const float bae = e ? ba.y : ba.x, bge = e ? bg.y : bg.x;
                                 if (ln) {
-                                    a = fmaf(a, ln_rs, fmaf(ln_nm, ua[j], ba[j]));
-                                    g = fmaf(g, ln_rs, fmaf(ln_nm, ug[j], bg[j]));
+                                    a = fmaf(a, ln_rs[h], fmaf(ln_nm[h], e ? ua.y : ua.x, bae));
+                                    gt = fmaf(gt, ln_rs[h], fmaf(ln_nm[h], e ? ug.y : ug.x, bge));
                                 } else {
-                                    a += ba[j];
-                                    g += bg[j];
+                                    a += bae;
+                                    gt += bge;
                                 }
-                                v[j] = a * gelu_tanh_f(g);
+                                v[e] = (valid[h] && o_base + 8 * i < n_out) ? a * gelu_tanh_f(gt) : 0.f;
                             }
-                            uint4 q;
-                            q.x = pack_bf16x2(v[0], v[1]);
-                            q.y = pack_bf16x2(v[2], v[3]);
-                            q.z = pack_bf16x2(v[4], v[5]);
-                            q.w = pack_bf16x2(v[6], v[7]);
-                            pk[2 * k + h8 / 8] = q;
+                            q[2 * g + h] = pack_bf16x2(v[0], v[1]);
                         }
                     }
+                    stmatrix_x4(s_out_addr + stage_off(st_row + st_j, 16 * k + 8 * st_grp), q[0], q[1], q[2], q[3]);
                 }
             } else if constexpr (MODE == 0 || MODE == 3 || MODE == 4 || MODE == 5) {
-                // lean path: per-row base pointers, 32-bit column offsets, uniform flags hoisted.
-                // The epilogue runs with only two warps per scheduler, so it is latency-bound unless
-                // the four 8-column groups of a chunk are independent straight-line code: the common
-                // case (tile fully inside the matrix, all 32 rows of the warp valid) has no per-group
-                // branches at all, and launches without residual / row-vector terms skip those adds.
+                // lean path: uniform flags hoisted. The epilogue runs with only two warps per scheduler, so it is
+                // latency-bound unless the 8-column groups are independent straight-line code: the common case (tile
+                // fully inside the matrix, all rows of the warp valid) has no per-group branches at all, and launches
+                // without residual / row-vector terms skip those adds.
                 if (etid == 0) GT(lt, 18);
                 const float alpha = effective_alpha(p);
                 const bool has_r1 = p.res1 != nullptr, has_r2 = p.res2 != nullptr, has_rv = p.rowvec != nullptr;
                 const int act = p.act;
-                const __nv_bfloat16* r1row = p.res1 + row * p.ldr1 + n_base;
-                const __nv_bfloat16* r2row = p.res2 + row * p.ldr2 + n_base;
-                const float* rvrow = p.rowvec + (int64_t)grp * p.rowvec_ld + n_base;
                 const int ncols = min(BLOCK_N, p.N - n_base);  // multiple of 8
-                const bool full = ncols == BLOCK_N && __all_sync(0xffffffffu, valid);
+                const bool full = ncols == BLOCK_N && __all_sync(0xffffffffu, valid[0] && valid[1]);
                 const bool plain = !has_r1 && !has_r2 && !has_rv;
-                if (etid == 0) GT(lt, 14);  // tile set-up done, about to run the main loop
-                mainloop(m_tile, n_tile);
-                if (etid == 0) GT(lt, 5);  // accumulator tile ready (epilogue thread 0)
-                // column split between the two warps sharing 32 rows: alternating 32-column chunks, except for the
-                // 160-wide tile (5 chunks would split 3 / 2): there each warp takes one contiguous 80-column half
-                // as 32 + 32 + 16, so both finish together
-                constexpr bool kSplitHalves = BLOCK_N == 160;
-                constexpr int NCH = kSplitHalves ? 3 : BLOCK_N / 64;  // chunks per thread (160: 32 + 32 + 16 columns)
-                auto chunk_col = [&](int k) { return kSplitHalves ? half * 80 + 32 * k : half * 32 + 64 * k; };
-                uint32_t accA[32], accB[32];
-                acc_ld(arow + chunk_col(0), accA);
-                // per-row partial sums for the consumer's LayerNorm (this warp's columns of the row): shifted by the
-                // first value seen so a large common offset does not cancel in the variance
-                constexpr bool want_rows = MODE == 3;  // mode 3 is only selected with row_stats set
-                // (packed fp32x2 arithmetic: three instructions per column pair)
-                uint64_t st_s1 = 0ull, st_s2 = 0ull;  // {even, odd} column lanes of sum and sum of squares
-                float st_shift = 0.f, st_cnt = 0.f;
-                // ---- store helper: 8 fp32 -> (silu) -> bf16 -> 16-byte store
-                auto store8 = [&](float (&v)[8], uint4& dst) {
-                    if (want_rows) {
-                        if (st_cnt == 0.f) st_shift = v[0];
-                        const uint64_t sh2 = pack_f32x2(st_shift, st_shift);
+                const bool ln_fold = MODE == 4 || (MODE == 5 && ln);  // these launches carry no residual / row vector
+                // residual and row-vector terms (only modes 0 / 3 carry them) of the column pair (8 i + 2 quad, + 1) of
+                // both rows, fetched D group pairs ahead of their use; the first D before the main loop's last wait. The
+                // 256-wide statistics producer has no registers for that: it fetches each pair's terms where it uses them
+                // (with D = 1 it would spill 614 bytes, more than the 506 of the fp32-tile epilogue).
+                constexpr bool kRes = MODE == 0 || MODE == 3;
+                constexpr int NP = BLOCK_N / 16;  // group pairs: one stmatrix.x4 each
+                constexpr int D = (MODE == 3 && BLOCK_N == 256) ? 0 : 1;
+                uint32_t q1[NP][2][2], q2[NP][2][2];  // [pair][group][row]
+                float2 tv[NP][2][2];
+                auto fetch = [&](int k) {
+                    if constexpr (kRes) {
+                        if (k >= NP) return;
 #pragma unroll
-                        for (int j = 0; j < 8; j += 2) {
-                            const uint64_t d = sub_f32x2(pack_f32x2(v[j], v[j + 1]), sh2);
-                            st_s1 = add_f32x2(st_s1, d);
-                            st_s2 = fma_f32x2(d, d, st_s2);
+                        for (int g = 0; g < 2; ++g) {
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int col = 16 * k + 8 * g;
+                                const bool ok = valid[h] && col < ncols;
+                                const int64_t c = n_base + col + 2 * quad;
+                                q1[k][g][h] = (ok && has_r1) ? __ldg(reinterpret_cast<const uint32_t*>(p.res1 + row[h] * p.ldr1 + c)) : 0u;
+                                q2[k][g][h] = (ok && has_r2) ? __ldg(reinterpret_cast<const uint32_t*>(p.res2 + row[h] * p.ldr2 + c)) : 0u;
+                                tv[k][g][h] = (ok && has_rv) ? __ldg(reinterpret_cast<const float2*>(p.rowvec + (int64_t)grp[h] * p.rowvec_ld + c))
+                                                             : make_float2(0.f, 0.f);
+                            }
                         }
-                        st_cnt += 8.f;
+                    }
+                };
+                if (etid == 0) GT(lt, 14);  // tile set-up done, about to run the main loop
+                mainloop(facc, m_tile, n_tile, [&] {
+#pragma unroll
+                    for (int k = 0; k < D; ++k) fetch(k);
+                });
+                if (etid == 0) GT(lt, 5);  // accumulators ready
+                if constexpr (kSplitK) {
+                    if (khalf) {
+                        // donor: the partial tile is in the workspace; publish it and leave (no output of its own)
+                        cp_async_wait_all();
+                        __threadfence();
+                        epi_sync();
+                        if (etid == 0) {
+                            __threadfence();
+                            *(volatile int32_t*)(p.splitk_flags + (int64_t)m_tile * n_tiles + n_tile) = 1;
+                        }
+                        continue;
+                    }
+                }
+                // mode 3: per row and half n-tile ([0, BLOCK_N / 2), [BLOCK_N / 2, BLOCK_N)) the sums of x - shift and
+                // (x - shift)^2, shift = the half's first value of the row (so a large common offset does not cancel in
+                // the variance)
+                float st_s1[2], st_s2[2], st_shift[2];
+                constexpr int HALF_NP = NP / 2;
+#pragma unroll
+                for (int k = 0; k < NP; ++k) {
+                    fetch(k + D);
+                    float v[2][2][2];  // [group][row][column of the pair]
+#pragma unroll
+                    for (int g = 0; g < 2; ++g) {
+                        const int i = 2 * k + g, c = 8 * i + 2 * quad;
+                        const float2 b = *reinterpret_cast<const float2*>(sbias + c);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const float a0 = facc[4 * i + 2 * h], a1 = facc[4 * i + 2 * h + 1];
+                            const bool ok = valid[h] && 8 * i < ncols;
+                            if (ln_fold) {
+                                const float2 u = *reinterpret_cast<const float2*>(su + c);
+                                // alpha == 1 for LayerNorm-folded launches (checked at prepare time)
+                                v[g][h][0] = ok ? fmaf(a0, ln_rs[h], fmaf(ln_nm[h], u.x, b.x)) : 0.f;
+                                v[g][h][1] = ok ? fmaf(a1, ln_rs[h], fmaf(ln_nm[h], u.y, b.y)) : 0.f;
+                            } else if (MODE == 4 || (full && plain)) {
+                                v[g][h][0] = (a0 + b.x) * alpha;
+                                v[g][h][1] = (a1 + b.y) * alpha;
+                            } else {
+                                const uint32_t r1 = kRes ? q1[k][g][h] : 0u, r2 = kRes ? q2[k][g][h] : 0u;
+                                const float2 t = kRes ? tv[k][g][h] : make_float2(0.f, 0.f);
+                                float x0 = a0 + b.x + t.x, x1 = a1 + b.y + t.y;
+                                x0 = (x0 + bf16_lo(r1)) * alpha + bf16_lo(r2);
+                                x1 = (x1 + bf16_hi(r1)) * alpha + bf16_hi(r2);
+                                v[g][h][0] = ok ? x0 : 0.f;
+                                v[g][h][1] = ok ? x1 : 0.f;
+                            }
+                        }
+                    }
+                    if constexpr (MODE == 3) {  // mode 3 is only selected with row_stats set, and without activation
+                        if (k % HALF_NP == 0) {
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                st_shift[h] = __shfl_sync(0xffffffffu, v[0][h][0], lane & ~3);
+                                st_s1[h] = st_s2[h] = 0.f;
+                            }
+                        }
+#pragma unroll
+                        for (int g = 0; g < 2; ++g) {
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                if (8 * (2 * k + g) < ncols) {
+#pragma unroll
+                                    for (int e = 0; e < 2; ++e) {
+                                        const float d = v[g][h][e] - st_shift[h];
+                                        st_s1[h] += d;
+                                        st_s2[h] = fmaf(d, d, st_s2[h]);
+                                    }
+                                }
+                            }
+                        }
+                        if (k % HALF_NP == HALF_NP - 1) {
+                            const int hf = k / HALF_NP;  // half n-tile
+                            const float cnt = (float)min(max(ncols - hf * (BLOCK_N / 2), 0), BLOCK_N / 2);
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                float s1 = st_s1[h], s2 = st_s2[h];
+                                s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+                                s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+                                s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+                                s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+                                if (quad == h && valid[h])
+                                    p.row_stats[(int64_t)(n_tile * 2 + hf) * p.row_stats_ld + row[h]] =
+                                        make_float4(s1, s2, st_shift[h], cnt);
+                            }
+                        }
                     }
                     if (act == PP_ACT_SILU) {
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = silu_f(v[j]);
+                        for (int j = 0; j < 8; ++j) (&v[0][0][0])[j] = silu_f((&v[0][0][0])[j]);
                     } else if (act == PP_ACT_QUICK_GELU) {
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = quick_gelu_f(v[j]);
+                        for (int j = 0; j < 8; ++j) (&v[0][0][0])[j] = quick_gelu_f((&v[0][0][0])[j]);
                     }
-                    uint4 q;
-                    if (MODE == 5 && ttile && p.t_fp16) {  // V^T is fp16 (P is fp16 in the attention kernel)
-                        q.x = pack_f16x2(v[0], v[1]);
-                        q.y = pack_f16x2(v[2], v[3]);
-                        q.z = pack_f16x2(v[4], v[5]);
-                        q.w = pack_f16x2(v[6], v[7]);
+                    if (MODE == 5 && ttile) {
+                        // transposed staging: [column][128 rows] 16-bit, 64-column sub-tiles of 16 KB (the boxes of the
+                        // transposed TMA store); V^T is fp16 (P is fp16 in the attention kernel). The layout is the TMA
+                        // box's and cannot be swizzled: the 16-byte rows of one stmatrix.trans are 256 bytes apart, so
+                        // its 512 bytes take 16 shared-memory wavefronts (a conflict-free store would take 4)
+                        uint32_t q[4];
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            q[j] = p.t_fp16 ? pack_f16x2(v[j >> 1][j & 1][0], v[j >> 1][j & 1][1])
+                                            : pack_bf16x2(v[j >> 1][j & 1][0], v[j >> 1][j & 1][1]);
+                        const int col = 16 * k + 8 * st_grp + st_j;
+                        stmatrix_x4_trans(s_out_addr + (col >> 6) * 16384 + (col & 63) * 256 + st_row * 2, q[0], q[1], q[2],
+                                          q[3]);
                     } else {
-                        q.x = pack_bf16x2(v[0], v[1]);
-                        q.y = pack_bf16x2(v[2], v[3]);
-                        q.z = pack_bf16x2(v[4], v[5]);
-                        q.w = pack_bf16x2(v[6], v[7]);
+                        stmatrix_x4(s_out_addr + stage_off(st_row + st_j, 16 * k + 8 * st_grp),
+                                    pack_bf16x2(v[0][0][0], v[0][0][1]), pack_bf16x2(v[0][1][0], v[0][1][1]),
+                                    pack_bf16x2(v[1][0][0], v[1][0][1]), pack_bf16x2(v[1][1][0], v[1][1][1]));
                     }
-                    dst = q;
-                };
-                // ---- one chunk of NG 8-column groups (32 or 16 columns); results go to pk[PKB + g]
-                auto process = [&](const uint32_t* accv, auto ng_tag, int c0, auto pkb_tag) {
-                    constexpr int NG = decltype(ng_tag)::value;
-                    constexpr int PKB = decltype(pkb_tag)::value;
-                    if (MODE == 4 || (MODE == 5 && ln)) {
-                        // LayerNorm-folded consumer (q|k, cross-attention q): acc' = rstd * (acc - mean * u[n]) + bias
-                        // fused as two FMAs; these launches carry no residual / row vector
-#pragma unroll
-                        for (int g = 0; g < NG; ++g) {
-                            const int col = c0 + g * 8;
-                            pk[PKB + g] = make_uint4(0u, 0u, 0u, 0u);
-                            if (valid && col < ncols) {
-                                const float4 b0 = *reinterpret_cast<const float4*>(sbias + col);
-                                const float4 b1 = *reinterpret_cast<const float4*>(sbias + col + 4);
-                                const float4 u0 = *reinterpret_cast<const float4*>(su + col);
-                                const float4 u1 = *reinterpret_cast<const float4*>(su + col + 4);
-                                float v[8];  // alpha == 1 for LayerNorm-folded launches (checked at prepare time)
-                                v[0] = fmaf(__uint_as_float(accv[g * 8 + 0]), ln_rs, fmaf(ln_nm, u0.x, b0.x));
-                                v[1] = fmaf(__uint_as_float(accv[g * 8 + 1]), ln_rs, fmaf(ln_nm, u0.y, b0.y));
-                                v[2] = fmaf(__uint_as_float(accv[g * 8 + 2]), ln_rs, fmaf(ln_nm, u0.z, b0.z));
-                                v[3] = fmaf(__uint_as_float(accv[g * 8 + 3]), ln_rs, fmaf(ln_nm, u0.w, b0.w));
-                                v[4] = fmaf(__uint_as_float(accv[g * 8 + 4]), ln_rs, fmaf(ln_nm, u1.x, b1.x));
-                                v[5] = fmaf(__uint_as_float(accv[g * 8 + 5]), ln_rs, fmaf(ln_nm, u1.y, b1.y));
-                                v[6] = fmaf(__uint_as_float(accv[g * 8 + 6]), ln_rs, fmaf(ln_nm, u1.z, b1.z));
-                                v[7] = fmaf(__uint_as_float(accv[g * 8 + 7]), ln_rs, fmaf(ln_nm, u1.w, b1.w));
-                                store8(v, pk[PKB + g]);
-                            }
-                        }
-                        return;
-                    }
-                    if constexpr (MODE != 4) {
-                    if (full && plain) {
-#pragma unroll
-                        for (int g = 0; g < NG; ++g) {
-                            const int col = c0 + g * 8;
-                            const float4 b0 = *reinterpret_cast<const float4*>(sbias + col);
-                            const float4 b1 = *reinterpret_cast<const float4*>(sbias + col + 4);
-                            float v[8];
-                            v[0] = (__uint_as_float(accv[g * 8 + 0]) + b0.x) * alpha; v[1] = (__uint_as_float(accv[g * 8 + 1]) + b0.y) * alpha;
-                            v[2] = (__uint_as_float(accv[g * 8 + 2]) + b0.z) * alpha; v[3] = (__uint_as_float(accv[g * 8 + 3]) + b0.w) * alpha;
-                            v[4] = (__uint_as_float(accv[g * 8 + 4]) + b1.x) * alpha; v[5] = (__uint_as_float(accv[g * 8 + 5]) + b1.y) * alpha;
-                            v[6] = (__uint_as_float(accv[g * 8 + 6]) + b1.z) * alpha; v[7] = (__uint_as_float(accv[g * 8 + 7]) + b1.w) * alpha;
-                            store8(v, pk[PKB + g]);
-                        }
-                        return;
-                    }
-                    // general: residuals / row vector / ragged tile. All loads of the chunk are issued
-                    // before any arithmetic so their latencies overlap.
-                    uint4 q1[NG], q2[NG];
-                    float4 t0[NG], t1[NG];
-                    bool ok[NG];
-#pragma unroll
-                    for (int g = 0; g < NG; ++g) {
-                        const int col = c0 + g * 8;
-                        ok[g] = valid && col < ncols;
-                        q1[g] = (ok[g] && has_r1) ? __ldg(reinterpret_cast<const uint4*>(r1row + col)) : make_uint4(0, 0, 0, 0);
-                        q2[g] = (ok[g] && has_r2) ? __ldg(reinterpret_cast<const uint4*>(r2row + col)) : make_uint4(0, 0, 0, 0);
-                        t0[g] = (ok[g] && has_rv) ? __ldg(reinterpret_cast<const float4*>(rvrow + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                        t1[g] = (ok[g] && has_rv) ? __ldg(reinterpret_cast<const float4*>(rvrow + col + 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-#pragma unroll
-                    for (int g = 0; g < NG; ++g) {
-                        const int col = c0 + g * 8;
-                        pk[PKB + g] = make_uint4(0u, 0u, 0u, 0u);
-                        if (ok[g]) {
-                            const float4 b0 = *reinterpret_cast<const float4*>(sbias + col);
-                            const float4 b1 = *reinterpret_cast<const float4*>(sbias + col + 4);
-                            float v[8];
-                            v[0] = __uint_as_float(accv[g * 8 + 0]) + b0.x + t0[g].x; v[1] = __uint_as_float(accv[g * 8 + 1]) + b0.y + t0[g].y;
-                            v[2] = __uint_as_float(accv[g * 8 + 2]) + b0.z + t0[g].z; v[3] = __uint_as_float(accv[g * 8 + 3]) + b0.w + t0[g].w;
-                            v[4] = __uint_as_float(accv[g * 8 + 4]) + b1.x + t1[g].x; v[5] = __uint_as_float(accv[g * 8 + 5]) + b1.y + t1[g].y;
-                            v[6] = __uint_as_float(accv[g * 8 + 6]) + b1.z + t1[g].z; v[7] = __uint_as_float(accv[g * 8 + 7]) + b1.w + t1[g].w;
-                            v[0] = (v[0] + bf16_lo(q1[g].x)) * alpha + bf16_lo(q2[g].x); v[1] = (v[1] + bf16_hi(q1[g].x)) * alpha + bf16_hi(q2[g].x);
-                            v[2] = (v[2] + bf16_lo(q1[g].y)) * alpha + bf16_lo(q2[g].y); v[3] = (v[3] + bf16_hi(q1[g].y)) * alpha + bf16_hi(q2[g].y);
-                            v[4] = (v[4] + bf16_lo(q1[g].z)) * alpha + bf16_lo(q2[g].z); v[5] = (v[5] + bf16_hi(q1[g].z)) * alpha + bf16_hi(q2[g].z);
-                            v[6] = (v[6] + bf16_lo(q1[g].w)) * alpha + bf16_lo(q2[g].w); v[7] = (v[7] + bf16_hi(q1[g].w)) * alpha + bf16_hi(q2[g].w);
-                            store8(v, pk[PKB + g]);
-                        }
-                    }
-                    }
-                };
-                using G4 = std::integral_constant<int, 4>;
-                using G2 = std::integral_constant<int, 2>;
-                // software pipeline over the chunks: the shared-memory load of chunk k + 1 is issued before chunk k is
-                // processed
-                auto chunk = [&](auto k_tag, uint32_t (&cur)[32], uint32_t (&nxt)[32]) {
-                    constexpr int K = decltype(k_tag)::value;
-                    if constexpr (K < NCH) {
-                        if constexpr (K + 1 < NCH) {
-                            if constexpr (kSplitHalves && K + 1 == 2) acc_ld(arow + chunk_col(K + 1), reinterpret_cast<uint32_t(&)[16]>(nxt));
-                            else acc_ld(arow + chunk_col(K + 1), nxt);
-                        }
-                        if constexpr (kSplitK) {
-                            // split-K: the donor's raw fp32 accumulators go to the workspace ([tile][row][BLOCK_N]); the
-                            // owner adds the donor's to its own (owner + donor, always in this order) before the epilogue
-                            constexpr int NQ = (kSplitHalves && K == 2) ? 4 : 8;  // float4 pieces of this chunk
-                            float4* wsp = reinterpret_cast<float4*>(
-                                p.splitk_ws + (((int64_t)m_tile * n_tiles + n_tile) * BLOCK_M + r) * BLOCK_N + chunk_col(K));
-                            if (khalf) {
-#pragma unroll
-                                for (int q = 0; q < NQ; ++q)
-                                    wsp[q] = make_float4(__uint_as_float(cur[4 * q]), __uint_as_float(cur[4 * q + 1]),
-                                                         __uint_as_float(cur[4 * q + 2]), __uint_as_float(cur[4 * q + 3]));
-                                return;
-                            }
-#pragma unroll
-                            for (int q = 0; q < NQ; ++q) {
-                                const float4 pp = __ldcg(wsp + q);
-                                cur[4 * q] = __float_as_uint(__uint_as_float(cur[4 * q]) + pp.x);
-                                cur[4 * q + 1] = __float_as_uint(__uint_as_float(cur[4 * q + 1]) + pp.y);
-                                cur[4 * q + 2] = __float_as_uint(__uint_as_float(cur[4 * q + 2]) + pp.z);
-                                cur[4 * q + 3] = __float_as_uint(__uint_as_float(cur[4 * q + 3]) + pp.w);
-                            }
-                        }
-#ifndef GEMM_EXP_NOEPI  // experiment: drain the accumulator only (what does the tile cost without the epilogue math?)
-                        if constexpr (kSplitHalves && K == 2) process(cur, G2{}, chunk_col(K), std::integral_constant<int, 4 * K>{});
-                        else process(cur, G4{}, chunk_col(K), std::integral_constant<int, 4 * K>{});
-#endif
-                    }
-                };
-                chunk(std::integral_constant<int, 0>{}, accA, accB);
-                chunk(std::integral_constant<int, 1>{}, accB, accA);
-                chunk(std::integral_constant<int, 2>{}, accA, accB);
-                chunk(std::integral_constant<int, 3>{}, accB, accA);
-                if constexpr (want_rows) {
-                    if (valid)
-                        p.row_stats[(int64_t)(n_tile * 2 + half) * p.row_stats_ld + row] =
-                            make_float4(f32x2_lo(st_s1) + f32x2_hi(st_s1), f32x2_lo(st_s2) + f32x2_hi(st_s2), st_shift, st_cnt);
                 }
             } else {
-                // residuals of a 32-column chunk are fetched one chunk ahead (the first chunk's
-                // before the main loop), so their latency hides behind the accumulator reads and
-                // the previous chunk's stores
+                // generic (fp32 / transposed / ragged N): straight from the fragment to global memory
                 const float alpha1 = effective_alpha(p);
-                uint4 c1[4], c2[4], x1[4], x2[4];
-                auto fetch = [&](int c0, uint4 (&a)[4], uint4 (&b)[4]) {
+                mainloop(facc, m_tile, n_tile, [] {});
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int n0 = n_base + c0 + g * 8;
-                        const bool ok = valid && vec_ok && c0 < BLOCK_N && n0 + 8 <= p.N;
-                        a[g] = (ok && p.res1) ? __ldg(reinterpret_cast<const uint4*>(p.res1 + row * p.ldr1 + n0))
-                                              : make_uint4(0, 0, 0, 0);
-                        b[g] = (ok && p.res2) ? __ldg(reinterpret_cast<const uint4*>(p.res2 + row * p.ldr2 + n0))
-                                              : make_uint4(0, 0, 0, 0);
-                    }
-                };
-                fetch(half * 32, c1, c2);
-                mainloop(m_tile, n_tile);
-#pragma unroll 1
-                for (int c0 = half * 32; c0 < BLOCK_N; c0 += 64) {
-                    fetch(c0 + 64, x1, x2);
-                    uint32_t accv[32];
-                    acc_ld(arow + c0, accv);
-                    if (valid) {
+                for (int i = 0; i < BLOCK_N / 8; ++i) {
 #pragma unroll
-                        for (int g = 0; g < 4; ++g) {
-                            const int n0 = n_base + c0 + g * 8;
-                            if (n0 < p.N) {
-                                float v[8];
+                    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(accv[g * 8 + j]);
-                                if (ln) {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) v[j] = fmaf(v[j], ln_rs, ln_nm * su[c0 + g * 8 + j]);
-                                }
-                                if (vec_ok && n0 + 8 <= p.N)
-                                    epilogue_store8<true>(p, alpha1, v, row, grp, n0, sbias + c0 + g * 8, c1[g], c2[g]);
-                                else
-                                    epilogue_store8<false>(p, alpha1, v, row, grp, n0, sbias + c0 + g * 8, c1[g], c2[g]);
+                        for (int e = 0; e < 2; ++e) {
+                            const int c = 8 * i + 2 * quad + e;
+                            if (valid[h] && n_base + c < p.N) {
+                                float v = facc[4 * i + 2 * h + e];
+                                if (ln) v = fmaf(v, ln_rs[h], ln_nm[h] * su[c]);
+                                epilogue_store1(p, alpha1, v, row[h], grp[h], n_base + c, sbias[c]);
                             }
                         }
                     }
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) { c1[g] = x1[g]; c2[g] = x2[g]; }
                 }
             }
-            // this thread's reads of the accumulator tile are complete: warpgroup 1 may take it over
-            if (etid == 0) GT(lt, 6);  // tile math done (results in registers)
-            if constexpr (kAccShared) {
-                if (wg == 0) asm volatile("bar.arrive 2, %0;" ::"n"(GEMM_EPI_WARPS * 32) : "memory");
-            }
+            if (etid == 0) GT(lt, 6);  // tile math done
             // the next tile's bias has landed in the other staging buffer (asynchronous copies issued at the top of this
             // tile); the barrier below publishes it before tile lt + 1 reads it
             cp_async_wait_all();
-            if constexpr (kSplitK) {
-                if (khalf) {
-                    // donor: the partial tile is in the workspace; publish it and leave (no output of its own)
-                    __threadfence();
-                    epi_sync();
-                    if (etid == 0) {
-                        __threadfence();
-                        *(volatile int32_t*)(p.splitk_flags + (int64_t)m_tile * n_tiles + n_tile) = 1;
-                    }
-                    continue;
-                }
-            }
             if constexpr (MODE == 3) {
                 if (etid == 0 && lt > 0) s_last_tile = ticket_verdict((int)lt);  // of tile lt - 1 (request number lt)
             }
+            if constexpr (MODE != 1) {
+                fence_proxy_async_smem();  // the staging stores (generic proxy) -> the TMA unit (async proxy)
+                if (quad == 0) {
+                    s_row[r0] = valid[0] ? (long long)row[0] : -1ll;
+                    s_row[r0 + 8] = valid[1] ? (long long)row[1] : -1ll;
+                }
+            }
             epi_sync();
-            if (etid == 0) GT(lt, 11);  // first barrier passed
+            if (etid == 0) GT(lt, 7);  // all epilogue warps staged
             // mode 3: the previous tile was the last n-tile of its row block -> fold the block's records (first four loads
             // now, the arithmetic after the hand-over to the TMA unit); then post this tile's ticket request
             float4 frc[4];
             bool fold_prev = false;
             if constexpr (MODE == 3) {
-                fold_prev = lt > 0 && s_last_tile != 0 && half == 0 && prev_valid;
+                fold_prev = lt > 0 && s_last_tile != 0 && prev_valid;
                 if (fold_prev) {
 #pragma unroll
                     for (int u = 0; u < 4; ++u)
@@ -1023,34 +888,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 }
             }
             if constexpr (MODE != 1) {
-                // stage the tile (generic-proxy writes -> async proxy), one barrier, one thread issues the TMA stores
-                // (one per sub-tile); the unit writes whole rows and clips out-of-range parts
-#pragma unroll
-                for (int i = 0; i < PK_N; ++i) {
-                    int col;
-                    if constexpr (MODE == 2) col = half * 16 + 32 * (i / 2) + 8 * (i % 2);
-                    else if constexpr (BLOCK_N == 160) col = half * 80 + 8 * i;
-                    else col = half * 32 + 64 * (i / 4) + 8 * (i % 4);
-                    if (MODE == 5 && ttile) {
-                        // transposed staging: [column][128 rows] 16-bit, 64-column sub-tiles of 16 KB — the boxes of the
-                        // transposed TMA store; a warp's 32 lanes write 64 contiguous bytes per column (conflict-free)
-                        uint8_t* tb = s_out + (col >> 6) * 16384 + (col & 63) * 256 + r * 2;
-                        const uint32_t w[4] = {pk[i].x, pk[i].y, pk[i].z, pk[i].w};
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            *reinterpret_cast<uint16_t*>(tb + (2 * j) * 256) = (uint16_t)(w[j] & 0xFFFFu);
-                            *reinterpret_cast<uint16_t*>(tb + (2 * j + 1) * 256) = (uint16_t)(w[j] >> 16);
-                        }
-                    } else {
-                        *reinterpret_cast<uint4*>(stage_ptr(r, col)) = pk[i];
-                    }
-                }
-                if (etid == 0) GT(lt, 12);  // staging stores issued
-                fence_proxy_async_smem();
-                if (etid == 0) GT(lt, 13);  // proxy fence done
-                if (half == 0) s_row[r] = valid ? (long long)row : -1ll;
-                epi_sync();
-                if (etid == 0) GT(lt, 7);  // all epilogue warps staged
                 constexpr int OUT_COLS = MODE == 2 ? BLOCK_N / 2 : BLOCK_N;
                 constexpr int PIECES = OUT_COLS / 8;
                 // one thread per 64-column sub-tile (lane 0 of the first warps) issues its store: a single thread issuing
@@ -1090,8 +927,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 }
                 if constexpr (MODE == 3) {
                     if (fold_prev) fold_row_records(frc, prev_row);
-                    prev_row = row;
-                    prev_valid = valid;
+                    prev_row = quad == 0 ? row[0] : row[1];
+                    prev_valid = quad < 2 && (quad == 0 ? valid[0] : valid[1]);
                 }
                 if constexpr (MODE == 0 || MODE == 3 || MODE == 4) {  // (never mode 5: transposed tiles hold no rows)
                     // GroupNorm partial sums of exactly the bf16 values the consumer will read
@@ -1110,7 +947,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                                 // it is the pixel-box origin of the sample / the sample's first row of the tile)
                                 float sh[8];
                                 {
-                                    const uint4 q = *reinterpret_cast<const uint4*>(stage_ptr(rb, piece * 8));
+                                    const uint4 q = *reinterpret_cast<const uint4*>(s_out + stage_off(rb, piece * 8));
                                     const bool okr = s_row[rb] >= 0;
                                     sh[0] = okr ? bf16_lo(q.x) : 0.f; sh[1] = okr ? bf16_hi(q.x) : 0.f;
                                     sh[2] = okr ? bf16_lo(q.y) : 0.f; sh[3] = okr ? bf16_hi(q.y) : 0.f;
@@ -1119,7 +956,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                                 }
                                 for (int rr = rb + l; rr < rb + seg_rows; rr += L) {
                                     if (s_row[rr] >= 0) {
-                                        const uint4 q = *reinterpret_cast<const uint4*>(stage_ptr(rr, piece * 8));
+                                        const uint4 q = *reinterpret_cast<const uint4*>(s_out + stage_off(rr, piece * 8));
                                         const float x[8] = {bf16_lo(q.x), bf16_hi(q.x), bf16_lo(q.y), bf16_hi(q.y),
                                                             bf16_lo(q.z), bf16_hi(q.z), bf16_lo(q.w), bf16_hi(q.w)};
 #pragma unroll
@@ -1144,7 +981,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             // the last tile's verdict and fold, then release the ticket server
             if (etid == 0 && lt > 0) s_last_tile = ticket_verdict((int)lt);
             epi_sync();
-            if (lt > 0 && s_last_tile != 0 && half == 0 && prev_valid) {
+            if (lt > 0 && s_last_tile != 0 && prev_valid) {
                 float4 frc[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u)
@@ -1435,8 +1272,8 @@ int gemm_stats_geometry(const pp_gemm_desc& d, pp_stats_geom* g) {
     return PP_OK;
 }
 
-// records per row a GEMM emits for the consumer's LayerNorm: one per half n-tile (the two epilogue warps that share a
-// row each own a set of columns); 0 = this launch cannot emit them
+// records per row a GEMM emits for the consumer's LayerNorm: one per half n-tile (columns [0, BLOCK_N / 2) and
+// [BLOCK_N / 2, BLOCK_N)); 0 = this launch cannot emit them
 int gemm_row_stats_records(const pp_gemm_desc& d0) {
     // the query comes before the record buffer exists: answer for the launch WITH row_stats attached (that one never
     // runs split-K, which can pick a different tile width and hence a different record count)
