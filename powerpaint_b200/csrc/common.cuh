@@ -86,6 +86,20 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
+// non-blocking probe of the same condition
+__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
 __device__ __forceinline__ uint64_t global_timer_ns() {
     uint64_t t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));

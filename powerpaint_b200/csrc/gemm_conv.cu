@@ -22,6 +22,8 @@
 //    of those rows. STAGES-deep smem ring with full/empty mbarriers that keeps running across tile boundaries, so the
 //    producer streams the next tile's operands while the consumers run this tile's epilogue. Each thread finishes its
 //    own accumulators in the wgmma fragment layout and writes the results to the output staging tile with stmatrix.
+//    Modes 0 / 3: the producer loads the tile's residual (res1) into that staging tile by TMA during the main loop,
+//    and the epilogue reads it back with ldmatrix where its stmatrix will write the result.
 //  * Split-K x2 (few tiles, long K): two CTAs per tile each stream half of K; the second hands its fp32 partial tile
 //    to the first through a global workspace (see the comment at the kernel).
 //  * Epilogue (fused): + bias[n] + time-embedding row vector + residual (skip / shortcut)
@@ -188,6 +190,14 @@ __device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t a, uin
                  : "memory");
 }
 
+// The inverse: lane l addresses row l % 8 of matrix l / 8, and gets back each matrix in the fragment layout.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+
 // Output staging tile: the epilogue writes its results (bf16) straight from the accumulator fragments (stmatrix) into
 // shared memory laid out as the boxes of a TMA store — 64-column sub-tiles [128 rows][128 B] with the 128-byte swizzle (the 160-wide tile ends in a
 // 32-column sub-tile [128][64 B] with the 64-byte swizzle) — and one thread per sub-tile hands them to the TMA unit,
@@ -247,12 +257,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
     const uint32_t s_out_addr = sB + STAGES * B_STAGE_BYTES;
     uint8_t* s_out = smem_raw + (s_out_addr - smem_u32(smem_raw));
     const uint32_t bar_base = s_out_addr + out_stage_bytes_for(BLOCK_N);
-    // barriers: full[STAGES], empty[STAGES]
+    // barriers: full[STAGES], empty[STAGES] (at most 8 each), then the residual staging pair: stage_free (every consumer
+    // warp is in the tile's main loop and its stores of the previous tile have read the staging tile) and res_full
+    // (the tile's residual boxes have landed in the staging tile)
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+    const uint32_t stage_free_bar = bar_base + 128u, res_full_bar = bar_base + 136u;
     // bias of the current / next tile, staged by the epilogue warps: [2][BLOCK_N] floats
     float* sbias_all = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw)));
-    // column sums of the gamma-folded weights (LayerNorm fold), staged like the bias: [2][BLOCK_N] floats
+    // column sums of the gamma-folded weights (LayerNorm fold) or, in modes 0 / 3, the tile's row-vector row (stage_rv),
+    // staged like the bias: [2][BLOCK_N] floats
     float* su_all = sbias_all + 2 * BLOCK_N;
     // validity of each tile row (statistics pass)
     long long* s_row = reinterpret_cast<long long*>(reinterpret_cast<uint8_t*>(sbias_all) + 4 * BLOCK_N * 4);
@@ -274,16 +288,26 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
     const int num_k_iters = p.num_k_iters;
     const int k_begin = split ? khalf * (num_k_iters / 2) : 0;
     const int k_end = split ? (khalf ? num_k_iters : num_k_iters / 2) : num_k_iters;
+    // modes 0 / 3: res1 reaches the epilogue through the staging tile (TMA during the main loop), and the time-embedding
+    // row vector through the second staging row (su_all, unused without the LayerNorm fold) when every tile lies in one
+    // sample; the split-K donor has no epilogue
+    constexpr bool kRes = MODE == 0 || MODE == 3;
+    const bool stage_res = kRes && p.res1 != nullptr && !(kSplitK && khalf);
+    const bool stage_rv =
+        kRes && p.rowvec != nullptr && (p.a_mode == PP_A_MATRIX ? p.rows_per_group % BLOCK_M == 0 : p.bn == 1);
 
     constexpr int W_PROD = GEMM_EPI_WARPS;
     if (warp == W_PROD && elect_one()) {
         prefetch_tmap(&p.tmA[0]);
         prefetch_tmap(&p.tmB);
         if constexpr (MODE != 1) prefetch_tmap(&p.tmOut[0]);
+        if (stage_res) prefetch_tmap(&p.tmRes[0]);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
             mbar_init(empty_bar(s), GEMM_EPI_WARPS);  // one arrival per consumer warp
         }
+        mbar_init(stage_free_bar, GEMM_EPI_WARPS);
+        mbar_init(res_full_bar, 1);
         fence_mbar_init();
         if constexpr (MODE == 3) { s_req_seq = 0; s_resp_seq = 0; s_req_mtile = 0; s_resp_last = 0; }
     }
@@ -331,6 +355,50 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             }
         }
         if (is_producer) {
+            // res1 of the producer's residual tile r_tile (local index r_lt) goes into the staging tile once stage_free
+            // says it is free, i.e. while the consumers run that tile's main loop: the same boxes and swizzles as the
+            // output store, so each value lands where the epilogue's stmatrix puts the result of its element.
+            // Out-of-bounds rows and columns read as zero; sub-tiles wholly beyond N are not loaded. The producer
+            // probes stage_free without blocking wherever it waits for a ring slot, so the operand stream never waits
+            // for the staging tile.
+            TileWalk rw(walk_first, walk_stride, n_tiles);
+            int r_tile = walk_first;
+            uint32_t r_lt = 0;
+            auto issue_res = [&] {
+                const int n_base = rw.n * BLOCK_N;
+                uint32_t bytes = 0;
+                for (int sub = 0; sub * 64 < BLOCK_N; ++sub)
+                    if (n_base + sub * 64 < p.N) bytes += (BLOCK_N - sub * 64) >= 64 ? 16384u : 8192u;
+                int x0 = 0, y0 = 0, nb0 = 0;
+                if (p.a_mode != PP_A_MATRIX) tile_origin(rw.m, x0, y0, nb0);
+                mbar_arrive_expect_tx(res_full_bar, bytes);
+                for (int sub = 0; sub * 64 < BLOCK_N && n_base + sub * 64 < p.N; ++sub) {
+                    const CUtensorMap* tm = (BLOCK_N - sub * 64) >= 64 ? &p.tmRes[0] : &p.tmRes[1];
+                    if (p.a_mode == PP_A_MATRIX)
+                        tma_load_2d(s_out_addr + sub * 16384, tm, res_full_bar, n_base + sub * 64, rw.m * BLOCK_M);
+                    else
+                        tma_load_4d(s_out_addr + sub * 16384, tm, res_full_bar, n_base + sub * 64, x0, y0, nb0);
+                }
+                rw.next();
+                r_tile += walk_stride;
+                ++r_lt;
+            };
+            auto poll_res = [&] {
+                while (r_tile < num_tiles && mbar_test_wait(stage_free_bar, r_lt & 1u)) issue_res();
+            };
+            auto wait_slot = [&](uint32_t bar, uint32_t parity) {
+                if (!stage_res) {
+                    mbar_wait(bar, parity);
+                    return;
+                }
+                poll_res();
+                const uint64_t t0 = global_timer_ns();
+                uint32_t spins = 0;
+                while (!mbar_test_wait(bar, parity)) {
+                    poll_res();
+                    if ((++spins & 0xFFu) == 0 && global_timer_ns() - t0 > PP_WAIT_TIMEOUT_NS) __trap();
+                }
+            };
             const int cpt = p.chunks0 + p.chunks1;  // chunks per tap
             int s = 0;                              // ring slot and its phase, carried across tiles
             uint32_t ph = 0;
@@ -347,7 +415,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                     kx = tap - ky * 3;
                 }
                 for (int it = k_begin; it < k_end; ++it) {
-                    mbar_wait(empty_bar(s), ph ^ 1u);
+                    wait_slot(empty_bar(s), ph ^ 1u);
                     if (it == k_begin) GT((tile - walk_first) / walk_stride, 0);
                     if (it == k_end - 1) GT((tile - walk_first) / walk_stride, 1);
 #if defined(GEMM_EXP_NOLOAD)  // experiment: no TMA traffic at all (operands are whatever the smem holds)
@@ -399,6 +467,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                     if (++s == STAGES) { s = 0; ph ^= 1u; }
                 }
             }
+            // the operands are all on their way: the residuals of the last tiles
+            if (stage_res) {
+                while (r_tile < num_tiles) {
+                    mbar_wait(stage_free_bar, r_lt & 1u);
+                    issue_res();
+                }
+            }
         }
     } else {
         // ===================== consumer warpgroups: MMA + epilogue =====================
@@ -434,6 +509,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 // one group stays in flight: the previous stage's MMAs have retired, its slot goes back to the producer
                 wgmma_wait<1>();
                 if (it > k_begin && lane_id() == 0) mbar_arrive(empty_bar(prev));
+                if (stage_res && it == k_begin) {
+                    // this warp is done with the staging tile of the previous tile (its stmatrix writes were fenced to
+                    // the async proxy before the store): once its stores have read it, the residual may go in
+                    __syncwarp();
+                    if (lane_id() == 0) {
+                        bulk_wait_read_all();
+                        mbar_arrive(stage_free_bar);
+                    }
+                }
                 prev = ks;
                 if (++ks == STAGES) { ks = 0; kph ^= 1u; }
             }
@@ -500,11 +584,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p.ln_u + n));
             return v;
         };
+        // row-vector row of an m-tile that lies in one sample (stage_rv)
+        auto rv_row = [&](int m_tile_of) -> const float* {
+            const int g = p.a_mode == PP_A_MATRIX ? m_tile_of * BLOCK_M / p.rows_per_group : m_tile_of / (p.tiles_x * p.tiles_y);
+            return p.rowvec + (int64_t)g * p.rowvec_ld;
+        };
         // stage the first tile's bias
         TileWalk tw(walk_first, walk_stride, n_tiles);
         if (walk_first < num_tiles) {
             const float b0 = load_bias(tw.n);
-            const float u0 = load_u(tw.n);
+            float u0 = load_u(tw.n);
+            if (stage_rv && etid < BLOCK_N && tw.n * BLOCK_N + etid < p.N) u0 = __ldg(rv_row(tw.m) + tw.n * BLOCK_N + etid);
             if (etid < BLOCK_N) {
                 sbias_all[etid] = b0;
                 su_all[etid] = u0;
@@ -585,6 +675,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 if (next_tile < num_tiles && p.bias && nn < p.N) cp_async_f32(db, p.bias + nn);
                 else *db = 0.f;
                 if (next_tile < num_tiles && ln && nn < p.N) cp_async_f32(du, p.ln_u + nn);
+                else if (next_tile < num_tiles && stage_rv && nn < p.N) cp_async_f32(du, rv_row(tw.m) + nn);
                 else *du = 0.f;
             }
             if (etid == 0) GT(lt, 16);
@@ -687,18 +778,34 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 const bool full = ncols == BLOCK_N && __all_sync(0xffffffffu, valid[0] && valid[1]);
                 const bool plain = !has_r1 && !has_r2 && !has_rv;
                 const bool ln_fold = MODE == 4 || (MODE == 5 && ln);  // these launches carry no residual / row vector
-                // residual and row-vector terms (only modes 0 / 3 carry them) of the column pair (8 i + 2 quad, + 1) of
-                // both rows, fetched D group pairs ahead of their use; the first D before the main loop's last wait. The
-                // 256-wide statistics producer has no registers for that: it fetches each pair's terms where it uses them
-                // (with D = 1 it would spill 614 bytes, more than the 506 of the fp32-tile epilogue).
-                constexpr bool kRes = MODE == 0 || MODE == 3;
+                // res1 comes from the staging tile and the row vector, where every tile lies in one sample, from su (both
+                // staged during the main loop). The other terms (res2, the row vector of tiles spanning two samples) of
+                // the column pair (8 i + 2 quad, + 1) of both rows are fetched D group pairs ahead of their use; the first
+                // D before the main loop's last wait. The 256-wide statistics producer has no registers for that: it
+                // fetches each pair's terms where it uses them (with D = 1 it spilled 614 bytes, more than the 506 of the
+                // fp32-tile epilogue).
                 constexpr int NP = BLOCK_N / 16;  // group pairs: one stmatrix.x4 each
                 constexpr int D = (MODE == 3 && BLOCK_N == 256) ? 0 : 1;
-                uint32_t q1[NP][2][2], q2[NP][2][2];  // [pair][group][row]
+                uint32_t q2[NP][2][2];  // [pair][group][row]
                 float2 tv[NP][2][2];
+                const bool fetch_rv = has_rv && !stage_rv;
+                // uniform: a launch without register-path terms skips their address arithmetic altogether (predicated
+                // off, it still took more than a third of each pair's instructions, in an issue-bound loop)
+                const bool reg_terms = has_r2 || fetch_rv;
                 auto fetch = [&](int k) {
                     if constexpr (kRes) {
                         if (k >= NP) return;
+                        if (!reg_terms) {
+#pragma unroll
+                            for (int g = 0; g < 2; ++g) {
+#pragma unroll
+                                for (int h = 0; h < 2; ++h) {
+                                    q2[k][g][h] = 0u;
+                                    tv[k][g][h] = make_float2(0.f, 0.f);
+                                }
+                            }
+                            return;
+                        }
 #pragma unroll
                         for (int g = 0; g < 2; ++g) {
 #pragma unroll
@@ -706,10 +813,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                                 const int col = 16 * k + 8 * g;
                                 const bool ok = valid[h] && col < ncols;
                                 const int64_t c = n_base + col + 2 * quad;
-                                q1[k][g][h] = (ok && has_r1) ? __ldg(reinterpret_cast<const uint32_t*>(p.res1 + row[h] * p.ldr1 + c)) : 0u;
                                 q2[k][g][h] = (ok && has_r2) ? __ldg(reinterpret_cast<const uint32_t*>(p.res2 + row[h] * p.ldr2 + c)) : 0u;
-                                tv[k][g][h] = (ok && has_rv) ? __ldg(reinterpret_cast<const float2*>(p.rowvec + (int64_t)grp[h] * p.rowvec_ld + c))
-                                                             : make_float2(0.f, 0.f);
+                                tv[k][g][h] = (ok && fetch_rv) ? __ldg(reinterpret_cast<const float2*>(p.rowvec + (int64_t)grp[h] * p.rowvec_ld + c))
+                                                               : make_float2(0.f, 0.f);
                             }
                         }
                     }
@@ -738,9 +844,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                 // the variance)
                 float st_s1[2], st_s2[2], st_shift[2];
                 constexpr int HALF_NP = NP / 2;
+                // staged residual: ldmatrix.x4 at the address of the pair's stmatrix.x4 returns it in fragment order
+                // (group g, row h in register 2 g + h), and the result goes back to the same place. A warp reads and
+                // writes only its own 16 rows.
+                auto st_addr = [&](int k) { return s_out_addr + stage_off(st_row + st_j, 16 * k + 8 * st_grp); };
+                if (stage_res) mbar_wait(res_full_bar, lt & 1u);
 #pragma unroll
                 for (int k = 0; k < NP; ++k) {
                     fetch(k + D);
+                    uint32_t r1q[4] = {0u, 0u, 0u, 0u};
+                    if (stage_res) ldmatrix_x4(st_addr(k), r1q);
                     float v[2][2][2];  // [group][row][column of the pair]
 #pragma unroll
                     for (int g = 0; g < 2; ++g) {
@@ -759,8 +872,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                                 v[g][h][0] = (a0 + b.x) * alpha;
                                 v[g][h][1] = (a1 + b.y) * alpha;
                             } else {
-                                const uint32_t r1 = kRes ? q1[k][g][h] : 0u, r2 = kRes ? q2[k][g][h] : 0u;
-                                const float2 t = kRes ? tv[k][g][h] : make_float2(0.f, 0.f);
+                                const uint32_t r1 = kRes ? r1q[2 * g + h] : 0u, r2 = kRes ? q2[k][g][h] : 0u;
+                                const float2 t = !kRes ? make_float2(0.f, 0.f)
+                                                 : stage_rv ? *reinterpret_cast<const float2*>(su + c) : tv[k][g][h];
                                 float x0 = a0 + b.x + t.x, x1 = a1 + b.y + t.y;
                                 x0 = (x0 + bf16_lo(r1)) * alpha + bf16_lo(r2);
                                 x1 = (x1 + bf16_hi(r1)) * alpha + bf16_hi(r2);
@@ -828,8 +942,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
                         stmatrix_x4_trans(s_out_addr + (col >> 6) * 16384 + (col & 63) * 256 + st_row * 2, q[0], q[1], q[2],
                                           q[3]);
                     } else {
-                        stmatrix_x4(s_out_addr + stage_off(st_row + st_j, 16 * k + 8 * st_grp),
-                                    pack_bf16x2(v[0][0][0], v[0][0][1]), pack_bf16x2(v[0][1][0], v[0][1][1]),
+                        stmatrix_x4(st_addr(k), pack_bf16x2(v[0][0][0], v[0][0][1]), pack_bf16x2(v[0][1][0], v[0][1][1]),
                                     pack_bf16x2(v[1][0][0], v[1][0][1]), pack_bf16x2(v[1][1][0], v[1][1][1]));
                     }
                 }
@@ -1479,6 +1592,23 @@ int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
                 rc = make_tmap_bf16_sw(&p.tmOut[k], d.out, 4, dims, str, box, k == 0 ? 128 : 64);
             }
             if (rc) return rc;
+            if ((l.mode == 0 || l.mode == 3) && d.res1) {
+                // the residual tile goes through the same boxes into the staging tile, so it lands where the
+                // epilogue's stmatrix writes the results
+                if (d.a_mode == PP_A_MATRIX) {
+                    uint64_t dims[2] = {(uint64_t)d.N, (uint64_t)d.M};
+                    uint64_t str[1] = {(uint64_t)d.ldr1 * 2};
+                    uint32_t box[2] = {inner, BLOCK_M};
+                    rc = make_tmap_bf16_sw(&p.tmRes[k], d.res1, 2, dims, str, box, k == 0 ? 128 : 64);
+                } else {
+                    uint64_t dims[4] = {(uint64_t)d.N, (uint64_t)p.wo, (uint64_t)p.ho, (uint64_t)p.nb};
+                    uint64_t str[3] = {(uint64_t)d.ldr1 * 2, (uint64_t)d.ldr1 * 2 * p.wo,
+                                       (uint64_t)d.ldr1 * 2 * p.wo * p.ho};
+                    uint32_t box[4] = {inner, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
+                    rc = make_tmap_bf16_sw(&p.tmRes[k], d.res1, 4, dims, str, box, k == 0 ? 128 : 64);
+                }
+                if (rc) return rc;
+            }
         }
     }
     if (d.chan_stats) {

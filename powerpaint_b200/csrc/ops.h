@@ -18,6 +18,7 @@ struct GemmKParams {
     CUtensorMap tmB;
     CUtensorMap tmOut[2];  // output tile store (modes 0 / 2): 64-column boxes, and the 32-column remainder box
     CUtensorMap tmOutT[2];  // mode 5: transposed tile store, boxes of 128 rows (tokens) x 64 / 32 channels
+    CUtensorMap tmRes[2];   // modes 0 / 3 with res1: tmOut's boxes over res1 (pitch ldr1), loaded into the staging tile
     int32_t trans_first_tile;  // mode 5: n-tiles from here on are stored transposed (into out_t)
     int32_t a_mode;
     int32_t M, N;            // GEMM extents (conv: M = nb*ho*wo)

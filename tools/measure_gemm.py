@@ -17,7 +17,10 @@ is compared with the first one (bit-identical, or rel-L2 of the sample).
 
 --trace reads the per-tile clocks a library built with PP_EXTRA_NVCC_FLAGS=-DGEMM_TRACE records for CTA 0 of the
 seeded run (`pp_debug_gemm_trace`): median SM clocks per tile of the main loop (slot 14 -> 5) and of the epilogue
-(slot 5 -> 10), for the epilogue flavours that record those slots (modes 0 / 3 / 4 / 5).
+(slot 5 -> 10), for the epilogue flavours that record those slots (modes 0 / 3 / 4 / 5). The epilogue is split into
+its fragment arithmetic and stmatrix, residual and row-vector waits included ("math", 5 -> 6), the staging barrier
+("stage", 6 -> 7; in mode 3 also the ticket verdict) and the TMA store issue, GroupNorm statistics pass and mode-3
+fold ("tail", 7 -> 10). Each is a median over the tiles on its own, so the parts need not add up to the epilogue.
 """
 from __future__ import annotations
 
@@ -138,17 +141,22 @@ def read_trace():
     # The buffer keeps entries of earlier launches, and clock64 is per SM (CTA 0 of another launch may have run on
     # another SM), so the tiles of this launch are the chain from tile 0 in which each tile starts right after the
     # previous one ended.
-    main, epi = [], []
+    main, epi, math, stage, tail = [], [], [], [], []
     for i, row in enumerate(t):
         if i and not 0 <= row[15] - t[i - 1][10] < 100_000:
             break
-        if not t[i][15] <= row[14] < row[5] < row[10]:
+        if not t[i][15] <= row[14] < row[5] <= row[6] <= row[7] <= row[10]:
             break
         main.append(row[5] - row[14])
         epi.append(row[10] - row[5])
+        math.append(row[6] - row[5])
+        stage.append(row[7] - row[6])
+        tail.append(row[10] - row[7])
     if not main:
         return None
-    return dict(tiles=len(main), main_clk=statistics.median(main), epi_clk=statistics.median(epi))
+    med = statistics.median
+    return dict(tiles=len(main), main_clk=med(main), epi_clk=med(epi), math_clk=med(math), stage_clk=med(stage),
+                tail_clk=med(tail))
 
 
 def child(configs, save_dir, trace):
@@ -282,7 +290,9 @@ def main():
         for pl in e["per_lib"]:
             if args.trace:
                 t = pl["trace"]
-                cells.append(f"main {t['main_clk']:8.0f} epi {t['epi_clk']:6.0f} clk ({t['tiles']} tiles)" if t else "no trace")
+                cells.append(f"main {t['main_clk']:8.0f} epi {t['epi_clk']:6.0f} = math {t['math_clk']:6.0f} + stage "
+                             f"{t['stage_clk']:6.0f} + tail {t['tail_clk']:6.0f} clk ({t['tiles']} tiles)"
+                             if t else "no trace")
             else:
                 cells.append(f"{pl['us_median']:8.1f} [{pl['us_min']:7.1f}, {pl['us_max']:7.1f}] µs {pl['tflops']:5.0f} TF "
                              f"{pl['sm_mhz_median']:5.0f} MHz")
