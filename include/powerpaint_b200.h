@@ -197,6 +197,10 @@ int32_t pp_gemm_row_stats_records(const pp_gemm_desc* d);
    It validates the shape and the tile width only: the answer is the launch's for a descriptor pp_gemm_conv accepts
    (e.g. row_stats together with ln_stats reports mode 3, while pp_gemm_conv refuses that descriptor) */
 pp_status pp_gemm_variant(const pp_gemm_desc* d, int32_t* block_n, int32_t* mode, int32_t* ksplit);
+/* host-only query: the epilogue terms this launch stages in shared memory during the main loop (modes 0 / 3): res1
+   through the output staging tile (*stage_res; the split-K donor half has no epilogue and stages nothing), the row
+   vector through the second staging row when every tile lies in one sample (*stage_rv). 1 = staged, 0 = not */
+pp_status pp_gemm_staging(const pp_gemm_desc* d, int32_t* stage_res, int32_t* stage_rv);
 
 /* ------------------------------------------------------------------ attention */
 typedef struct pp_attn_desc {

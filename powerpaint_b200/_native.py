@@ -161,6 +161,7 @@ _SIGNATURES = {
     "pp_gemm_row_stats_records": (i32, [C.POINTER(GemmDesc)]),
     "pp_gemm_splitk_bytes": (i64, [C.POINTER(GemmDesc), C.POINTER(i32)]),
     "pp_gemm_variant": (C.c_int, [C.POINTER(GemmDesc), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
+    "pp_gemm_staging": (C.c_int, [C.POINTER(GemmDesc), C.POINTER(i32), C.POINTER(i32)]),
     "pp_attention": (C.c_int, [C.POINTER(AttnDesc), vp]),
     "pp_attention_variant": (C.c_int, [C.POINTER(AttnDesc), C.POINTER(i32), C.POINTER(i32)]),
     "pp_group_norm": (C.c_int, [C.POINTER(GnDesc), vp]),

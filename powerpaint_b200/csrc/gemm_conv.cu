@@ -1091,7 +1091,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_conv_kernel(const __grid
             if (etid == 0) GT(lt, 10);
         }
         if constexpr (MODE == 3) {
-            // the last tile's verdict and fold, then release the ticket server
+            // the last tile's verdict and fold, then release the ticket server. The barrier first: every warp has read
+            // the previous verdict (fold_prev, after the last tile's second barrier) before etid 0 overwrites it
+            epi_sync();
             if (etid == 0 && lt > 0) s_last_tile = ticket_verdict((int)lt);
             epi_sync();
             if (lt > 0 && s_last_tile != 0 && prev_valid) {
@@ -1422,6 +1424,20 @@ int gemm_variant(const pp_gemm_desc& d, int* block_n, int* mode, int* ksplit) {
     return PP_OK;
 }
 
+static int gemm_staging(const pp_gemm_desc& d, int* stage_res, int* stage_rv) {
+    GemmKParams p;
+    memset(&p, 0, sizeof(p));
+    int bn = 0;
+    int rc = gemm_geometry(d, p, &bn);
+    if (rc) return rc;
+    // the kernel's stage_res / stage_rv of a launch (the split-K donor's half stages nothing: it has no epilogue)
+    const int mode = gemm_select_mode(d);
+    const bool kRes = mode == 0 || mode == 3;
+    *stage_res = kRes && d.res1 != nullptr;
+    *stage_rv = kRes && d.rowvec != nullptr && (d.a_mode == PP_A_MATRIX ? d.rows_per_group % BLOCK_M == 0 : p.bn == 1);
+    return PP_OK;
+}
+
 int gemm_prepare(const pp_gemm_desc& d, GemmLaunch* out) {
     GemmLaunch l;
     memset(&l, 0, sizeof(l));
@@ -1695,6 +1711,19 @@ extern "C" pp_status pp_gemm_variant(const pp_gemm_desc* d, int32_t* block_n, in
     *block_n = bn;
     *mode = m;
     *ksplit = ks;
+    return pp::PP_OK;
+}
+
+extern "C" pp_status pp_gemm_staging(const pp_gemm_desc* d, int32_t* stage_res, int32_t* stage_rv) {
+    if (!d || !stage_res || !stage_rv) {
+        pp::set_last_error("pp_gemm_staging: null argument");
+        return pp::PP_ERR_INVALID;
+    }
+    int r = 0, v = 0;
+    int rc = pp::gemm_staging(*d, &r, &v);
+    if (rc) return rc;
+    *stage_res = r;
+    *stage_rv = v;
     return pp::PP_OK;
 }
 

@@ -181,6 +181,14 @@ def gemm_variant(desc: Desc):
     return int(bn.value), int(mode.value), int(ks.value)
 
 
+def gemm_staging(desc: Desc):
+    """host-only: (res1 staged, row vector staged): the epilogue terms this launch stages in shared memory during the
+    main loop"""
+    r, v = N.i32(0), N.i32(0)
+    N.check(N.lib().pp_gemm_staging(C.byref(desc.c), C.byref(r), C.byref(v)), "pp_gemm_staging")
+    return bool(r.value), bool(v.value)
+
+
 def attention_variant(desc: Desc):
     """host-only: (dv, p_fp16) of the kernel variant pp_attention would launch for this descriptor"""
     dv, f16 = N.i32(0), N.i32(0)

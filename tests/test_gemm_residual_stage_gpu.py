@@ -119,8 +119,15 @@ def test_staged_epilogue_terms(ops, cid, variant, route, spec):
     desc, t, outs, canv, extra, fill, keep = _prepare(spec, variant, seed=sum(map(ord, cid)))
     d = desc.c
     assert ops.gemm_variant(desc) == variant, (cid, ops.gemm_variant(desc))
+    staged = ops.gemm_staging(desc)
+    assert staged[0] == bool(spec.get("res1")), (cid, staged)  # res1 goes through the staging tile
     if route:
         reg = _register_route(ops, desc, t, route, keep)
+        # the route under comparison takes the register path for the term this case stages
+        if route == "res2":
+            assert staged[0] and not ops.gemm_staging(reg)[0], cid
+        else:
+            assert staged[1] and not ops.gemm_staging(reg)[1], cid
         want = _run(ops, reg, outs, extra, fill)
     got = _run(ops, desc, outs, extra, fill)
     worst = kv.check_gemm(cid, d, t, outs, canv, variant[0])
