@@ -44,6 +44,9 @@
  *   pp_softmax_rows, pp_image_preprocess_u8, pp_image_postprocess   VAE attention softmax and the uint8
  *                     pre/post-processing either side of vae.encode / vae.decode
  *                     (pipeline_PowerPaint.py:39-153,657-669,1051,1062)
+ *   pp_resample_u8, pp_box_blur_u8, pp_canny_u8, pp_outpaint_canvas_u8, pp_app_blend_u8   the app's request
+ *                     pre / post-processing (Pillow resize and GaussianBlur, cv2.Canny, canvas and blends;
+ *                     app.py:258-387,405-473); pp_gaussian_box_radius, pp_canny_workspace_bytes host-only
  *   pp_window_copy, pp_tile_blend   tiled VAE encode / decode (diffusers AutoencoderKL.enable_tiling,
  *                     pipeline_PowerPaint_ControlNet.py:341-356): tile gather / assembly and the seam blend
  *   pp_embed_gather, pp_causal_attention_small   CLIP text encoder: embeddings with the task-prompt splice
@@ -293,6 +296,44 @@ pp_status pp_image_preprocess_u8(const uint8_t* image, const void* mask, int32_t
    and / or fp32 NCHW [nb,3,hw] — `VaeImageProcessor.postprocess` (pipeline_PowerPaint.py:1062) */
 pp_status pp_image_postprocess(const void* x, int32_t x_is_fp32, int32_t c_ld, uint8_t* out_u8, float* out_f32,
                                int32_t nb, int32_t hw, pp_stream stream);
+
+/* ------------------------------------------------------------------ the app's request pre / post-processing */
+/* All images are uint8 HWC with 1 or 3 channels; each result equals the library named, byte for byte
+   (ref:app.py:258-387,405-473). */
+/* Pillow Image.resize (modes L / RGB): a horizontal pass when out_w != in_w, then a vertical one when
+   out_h != in_h (a copy when neither). The host builds each axis's tables as Pillow does: bounds [out * 2] =
+   (first source pixel, tap count), k [out * taps] = weights in 22-bit fixed point. A two-pass resize writes its
+   horizontal result to tmp [in_h, out_w, channels]. */
+pp_status pp_resample_u8(const uint8_t* src, uint8_t* tmp, uint8_t* dst, int32_t in_h, int32_t in_w, int32_t out_h,
+                         int32_t out_w, int32_t channels, const int32_t* bounds_x, const int32_t* k_x, int32_t taps_x,
+                         const int32_t* bounds_y, const int32_t* k_y, int32_t taps_y, pp_stream stream);
+/* host-only: the extended box radius Pillow's GaussianBlur(radius) runs `passes` passes of per axis */
+float pp_gaussian_box_radius(float radius, int32_t passes);
+/* Pillow's extended box blur: `passes` horizontal then `passes` vertical passes, edges replicated; tmp is an
+   image-sized scratch buffer distinct from src and dst. GaussianBlur(r) = pp_box_blur_u8 with
+   pp_gaussian_box_radius(r, 3) and 3 passes. */
+pp_status pp_box_blur_u8(const uint8_t* src, uint8_t* tmp, uint8_t* dst, int32_t h, int32_t w, int32_t channels,
+                         float box_radius, int32_t passes, pp_stream stream);
+/* host-only: workspace bytes pp_canny_u8 needs for an h x w image (-1 for a zero size) */
+int64_t pp_canny_workspace_bytes(int32_t h, int32_t w);
+/* cv2.Canny(src, low, high) with aperture 3 and the L1 norm -> dst [h, w] in {0, 255}. Five launches: Sobel,
+   suppression + tile-local union-find, tile merge, root marking, output; no host synchronisation. */
+pp_status pp_canny_u8(const uint8_t* src, uint8_t* dst, void* workspace, int64_t workspace_bytes, int32_t h, int32_t w,
+                      int32_t channels, double low, double high, pp_stream stream);
+/* The outpainting canvas: img = 127 with src [o_h, o_w, 3] at (top, left); mask = 255 except 0 in rows
+   [hole_y0, hole_y1) x columns [hole_x0, hole_x1) (an empty range leaves it all 255). Both RGB [c_h, c_w, 3]. */
+pp_status pp_outpaint_canvas_u8(const uint8_t* src, int32_t o_h, int32_t o_w, uint8_t* img, uint8_t* mask,
+                                int32_t c_h, int32_t c_w, int32_t top, int32_t left, int32_t hole_y0, int32_t hole_y1,
+                                int32_t hole_x0, int32_t hole_x1, pp_stream stream);
+/* Per-pixel steps over RGB a [h, w, 3] and a mask b [h, w, b_channels] (1 or 3), float64 in NumPy's operation order,
+   truncated to uint8:
+     PP_BLEND_LUMA         out [h, w, 1] = Pillow's RGB -> L of a (b, c unused)
+     PP_BLEND_HOLE_FILL    out = a * (1 - b / 255.0)                                  (the v2 hole fill)
+     PP_BLEND_RED_OVERLAY  out = a * (1 - b / 512.0) + b / 512.0 * (180, 0, 0)
+     PP_BLEND_PASTE        out = (a / 255.0 * (b / 255.0) + (1 - b / 255.0) * (c / 255.0)) * 255, c RGB */
+enum { PP_BLEND_LUMA = 0, PP_BLEND_HOLE_FILL = 1, PP_BLEND_RED_OVERLAY = 2, PP_BLEND_PASTE = 3 };
+pp_status pp_app_blend_u8(int32_t op, const uint8_t* a, const uint8_t* b, const uint8_t* c, uint8_t* out, int32_t h,
+                          int32_t w, int32_t b_channels, pp_stream stream);
 
 /* ------------------------------------------------------------------ tiled VAE (diffusers enable_tiling) */
 /* One rectangular window of pixels: `rows` x `cols` pixels starting at element offset src_off of the source and

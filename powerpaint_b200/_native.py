@@ -19,6 +19,7 @@ _lib = None
 PP_A_MATRIX, PP_A_CONV3X3, PP_A_CONV3X3_S2, PP_A_CONV3X3_S2P0 = 0, 1, 2, 3
 PP_EPI_PLAIN, PP_EPI_GEGLU, PP_EPI_TRANSPOSED, PP_EPI_ROWS_THEN_TRANSPOSED = 0, 1, 2, 3
 PP_ACT_NONE, PP_ACT_SILU, PP_ACT_QUICK_GELU = 0, 1, 2
+PP_BLEND_LUMA, PP_BLEND_HOLE_FILL, PP_BLEND_RED_OVERLAY, PP_BLEND_PASTE = 0, 1, 2, 3
 ABI_VERSION = 5
 
 vp = C.c_void_p
@@ -187,6 +188,13 @@ _SIGNATURES = {
     "pp_program_add_causal_attention_small": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, f32]),
     "pp_image_preprocess_u8": (C.c_int, [vp, vp, i32, vp, i32, i32, i32, f32, f32, vp]),
     "pp_image_postprocess": (C.c_int, [vp, i32, i32, vp, vp, i32, i32, vp]),
+    "pp_resample_u8": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, vp]),
+    "pp_gaussian_box_radius": (f32, [f32, i32]),
+    "pp_box_blur_u8": (C.c_int, [vp, vp, vp, i32, i32, i32, f32, i32, vp]),
+    "pp_canny_workspace_bytes": (i64, [i32, i32]),
+    "pp_canny_u8": (C.c_int, [vp, vp, vp, i64, i32, i32, i32, C.c_double, C.c_double, vp]),
+    "pp_outpaint_canvas_u8": (C.c_int, [vp, i32, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
+    "pp_app_blend_u8": (C.c_int, [i32, vp, vp, vp, vp, i32, i32, i32, vp]),
     "pp_program_add_softmax_rows": (C.c_int, [vp, vp, vp, i64, i32, i64, i64]),
     "pp_window_copy": (C.c_int, [vp, vp, i32, i32, i64, i64, vp, i32, i32, vp]),
     "pp_program_add_window_copy": (C.c_int, [vp, vp, vp, i32, i32, i64, i64, vp, i32, i32]),
