@@ -15,6 +15,7 @@ powerpaint/pipelines/pipeline_PowerPaint.py:657-669, decode :1051; pipeline_Powe
   Upsample2D: nearest 2x + conv                         pp_upsample_nearest + conv
   mid-block Attention, 1 head x 512 channels            to_q|to_k GEMM + V^T GEMM, then per sample
                                                         S = QK^T (fp32) -> pp_softmax_rows -> O = PV, to_out(+res)
+                                                        (O in chains of 2048-key GEMMs above 4096 keys)
   conv_out -> quant_conv (1x1)                          folded on the host into ONE 3x3 conv (exact: both linear)
   post_quant_conv (1x1) -> conv_in                      1x1 GEMM, then conv (not folded: the bias meets zero padding)
 
@@ -105,6 +106,31 @@ def vae_param_shapes(in_channels=3, out_channels=3, latent_channels=4, block_out
 # --------------------------------------------------------------------------- tile geometry
 # Attention S = QK^T of one image is a [hw, hw] fp32 matrix and pp_softmax_rows takes at most 16384 columns
 VAE_MAX_LATENT_PIXELS = 16384
+# O = P V sums over all hw keys. The tensor cores' fp32 accumulation error grows with the number of k-steps, and on
+# softmax weights (all non-negative) it does not cancel: above PV_K_SINGLE keys the product runs as a chain of GEMMs
+# over PV_K_CHUNK keys each, every one adding the fp32 sum of the chunks before it through its row vector
+PV_K_SINGLE = 4096
+PV_K_CHUNK = 2048
+
+
+def add_pv_product(prog, p: torch.Tensor, vt: torch.Tensor, out: torch.Tensor,
+                   partial: Optional[Tuple[torch.Tensor, torch.Tensor]]) -> None:
+    """record out = P V: p bf16 [hw, k_ld], vt bf16 [C, k_ld] (both with every one of the k_ld keys readable), out bf16
+    [hw, C]. Above PV_K_SINGLE keys `partial` holds two fp32 [hw, C] buffers the chain's running sums alternate in."""
+    hw, k_ld = p.shape
+    C = vt.shape[0]
+    if k_ld <= PV_K_SINGLE:
+        prog.add(ops.gemm_desc(a0=p, c0=k_ld, lda0=k_ld, w=vt, ldb=k_ld, out=out, N_=C, M=hw))
+        return
+    prev = None
+    for j, k0 in enumerate(range(0, k_ld, PV_K_CHUNK)):
+        k1 = min(k_ld, k0 + PV_K_CHUNK)
+        last = k1 == k_ld
+        dst = out if last else partial[j % 2]
+        prog.add(ops.gemm_desc(a0=p[:, k0:], c0=k1 - k0, lda0=k_ld, w=vt[:, k0:], ldb=k_ld, out=dst, N_=C, M=hw,
+                               rowvec=prev, rows_per_group=1 if prev is not None else 0,
+                               rowvec_ld=C if prev is not None else 0, out_fp32=not last))
+        prev = dst
 
 
 @dataclass(frozen=True)
@@ -216,14 +242,17 @@ class VaeEngine(Recorder):
                                epilogue=N.PP_EPI_TRANSPOSED, t_rows=hw, t_ld=hw_ld))
         plan.pool.free(g)
         o = plan.pool.buf(M, C)
+        partial = None
+        if hw_ld > PV_K_SINGLE:
+            partial = (plan.pool.buf(hw, C, dtype=torch.float32), plan.pool.buf(hw, C, dtype=torch.float32))
         scale = 1.0 / math.sqrt(C)
         for b in range(nb):
             rows = qk[b * hw:(b + 1) * hw]
             prog.add(ops.gemm_desc(a0=rows, c0=C, lda0=2 * C, w=rows[:, C:], ldb=2 * C, out=sm, N_=hw, M=hw, alpha=scale,
                                    out_fp32=True))
             prog.add_softmax_rows(sm, pm, hw, hw, hw, hw_ld)
-            prog.add(ops.gemm_desc(a0=pm, c0=hw_ld, lda0=hw_ld, w=vt[b], ldb=hw_ld, out=o[b * hw:(b + 1) * hw], N_=C, M=hw))
-        plan.pool.free(qk, vt, pm, sm)
+            add_pv_product(prog, pm, vt[b], o[b * hw:(b + 1) * hw], partial)
+        plan.pool.free(qk, vt, pm, sm, *(partial or ()))
         out = self._linear(plan, prog, o, M, name + ".to_out.0", C, bias=self.vec(name + ".to_out.0.bias"), res1=x,
                            stats_hw=hw)
         plan.pool.free(o)
